@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — IDM-VTON denoising hot path on B200: try-on images/sec @768x1024, 30 steps, CFG 2.0 (BASELINE.json).
+"""bench.py — IDM-VTON denoising hot path on H100: try-on images/sec @768x1024, 30 steps, CFG 2.0 (BASELINE.json).
 
 One bench "step" = one pass of the hot path over one batch: the full 30-step denoising loop
 (src/tryon_pipeline.py:1765-1866: garment UNet + try-on UNet + CFG + DDPM per denoise step) for `batch` try-on
@@ -116,23 +116,19 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return dict(tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1400.0))),
-                    tflops_burst=float(d.get("bf16_tflops", 1590.0)), hbm=float(d.get("hbm_gbs", 6650.0)),
+        return dict(tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0))),
+                    tflops_burst=float(d.get("bf16_tflops", 989.0)), hbm=float(d.get("hbm_gbs", 3350.0)),
                     source="measured (MEASURED_PEAKS.json: burst bf16 for the kernel timed alone, sustained for the loop)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet, dense bf16 at a 700 W limit; not reached by any measured kernel
+    return dict(tflops=989.0, tflops_burst=989.0, hbm=3350.0, source="fallback (H100 SXM data sheet, 700 W)")
 
 
-# DRAM traffic of one launch of the dominant kernel shape, from `ncu --set full` (dram__bytes_read.sum +
-# dram__bytes_write.sum; profiles/r2_ncu_summary.json, same numbers as round 1's capture). Algorithmic bytes of that launch:
-# A 7.9 MB + W 26.2 MB + out 31.5 MB = 65.5 MB.
-DOMINANT_KERNEL_DRAM_BYTES = 37605120   # 34.15 MB read + 3.46 MB written: the 31.5 MB output stays in the 126 MB L2
-DOMINANT_KERNEL_TRAFFIC_SOURCE = "profiles/r2_ncu_summary.json (ncu --set full, one launch after an L2 flush; config-2 shape)"
 
 
 def time_dominant_kernel(device, rows, n=20):
     """Live CUDA-event timing of the dominant kernel on its largest launch: the GEGLU feed-forward GEMM of the 60
     C=1280 transformer blocks ([rows x 10240 x 1280] with rows = 2*batch*tokens of the 1/4-resolution level,
-    gemm2_kernel<256,5,GEGLU>), L2 flushed between launches."""
+    gemm_conv_kernel<256, GEGLU>), L2 flushed between launches."""
     from idm_vton_b200 import lib as L
     from idm_vton_b200.engine import pack_geglu
     M, N, K = rows, 10240, 1280
@@ -156,8 +152,9 @@ def time_dominant_kernel(device, rows, n=20):
         ms.append(s.elapsed_time(e))
     avg = sum(ms) / len(ms)
     flops = 2.0 * M * N * K
-    return dict(kernel=f"gemm2_kernel<BN=256,STAGES=5,GEGLU> [{M}x{N}x{K}] (FF1 of the C=1280 transformer blocks, "
-                       "2-CTA tcgen05 GEMM family)", ms=avg, n=n, flops=flops, tflops=flops / avg / 1e9, rows=M)
+    return dict(kernel=f"gemm_conv_kernel<BN=256,STAGES=4,GEGLU> [{M}x{N}x{K}] (FF1 of the C=1280 transformer blocks, "
+                       "wgmma GEMM)", ms=avg, n=n, flops=flops, tflops=flops / avg / 1e9, rows=M,
+                bytes=2.0 * (M * K + N * K + M * N // 2))
 
 
 class ClockSampler:
@@ -372,7 +369,7 @@ def run_reference(args, rank, world):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# engine arm
 # ------------------------------------------------------------------------------------------------
 def build_components(device, rank, world, log):
     """Both UNets on every rank. The weights live in one flat arena per UNet (parallel.alloc_state_dict_arena); rank 0
@@ -419,7 +416,7 @@ def make_pipeline(unet, unet_enc, device):
     from idm_vton_b200.vae import AutoencoderKL
     torch.manual_seed(0)
     vae = AutoencoderKL().to(device, torch.float16).eval()
-    # CLIP ViT-H/14 geometry of /root/reference/ckpt/image_encoder/config.json, random init (no checkpoints offline)
+    # CLIP ViT-H/14 geometry of the reference's ckpt/image_encoder/config.json, random init (no checkpoints offline)
     ccfg = CLIPVisionConfig(hidden_size=1280, intermediate_size=5120, num_hidden_layers=32, num_attention_heads=16,
                             patch_size=14, image_size=224, projection_dim=1024)
     image_encoder = CLIPVisionModelWithProjection(ccfg).to(device, torch.float16).eval()
@@ -433,7 +430,7 @@ def eager_gpu_baseline(cfg, unet, unet_enc, device, log):
     """The reference's arithmetic as eager PyTorch on the SAME GPU: the oracle (oracle/unet_ref.py + loop_ref.py) under
     torch.autocast(fp16) with fp16 weights — the reference's own execution mode (inference.py:223,339) with stock ATen /
     cuBLAS / cuDNN / SDPA kernels. One full denoise step of the workload batch, timed after one warm-up; images/sec =
-    batch / (denoise_steps * t_step). Informational (BASELINE.md section 4): the reference has no Blackwell kernels of its own."""
+    batch / (denoise_steps * t_step). Informational (BASELINE.md section 4): the reference has no native GPU kernels of its own."""
     from oracle import loop_ref as LR
     from oracle import unet_ref as R
     B, Bg, h, w, T = cfg["batch"], cfg["garments"], cfg["height"] // 8, cfg["width"] // 8, cfg["denoise_steps"]
@@ -452,6 +449,21 @@ def eager_gpu_baseline(cfg, unet, unet_enc, device, log):
     return {"value": B / (T * t_step), "unit": "images/s", "ms_per_denoise_step": t_step * 1e3,
             "what": "oracle port of the reference loop under torch.autocast(fp16) on this GPU (ATen/cuBLAS/cuDNN/SDPA), "
                     f"1 denoise step of batch {B} timed (best of 2 after warm-up), x {T} steps; loop only"}
+
+
+def dump_outputs(directory, arrays, limit_bytes=64 << 20):
+    """Writes what the timed path returned in its last step as <directory>/<name>.npy (float32), so that two builds can be
+    compared output for output. The inputs are seeded, so the same arguments give the same inputs on every run. An array
+    over the size limit is replaced by a fixed, seeded sample of its elements."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    budget = limit_bytes // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget:
+            idx = np.random.default_rng(0).choice(a.size, budget // 4, replace=False)
+            a = a.reshape(-1)[np.sort(idx)]
+        np.save(os.path.join(directory, f"{name}.npy"), a.astype(np.float32))
 
 
 def run_b200(args, rank, world, local):
@@ -497,11 +509,12 @@ def run_b200(args, rank, world, local):
             if den.hoist_garment:
                 den.precompute_garment(0)    # the garment-UNet passes of this request (batched) + garment K/V
             return denoise(reqs[0])
+        outs = []
         for req in reqs:
             den.prepare(**req, guidance_scale=GUIDANCE)
             den.set_step_tables(sch, sch.timesteps)        # includes the hoisted garment passes
-            out = denoise(req)
-        return out
+            outs.append(denoise(req).clone())              # den.latents is reused by the next batch
+        return outs[-1] if len(outs) == 1 else torch.cat(outs, 0)
 
     den.prepare(**reqs[0], guidance_scale=GUIDANCE)
     den.set_step_tables(sch, sch.timesteps)
@@ -540,7 +553,7 @@ def run_b200(args, rank, world, local):
     with ClockSampler(local) as clocks:
         for s, e in evs:
             s.record()
-            run_loop()
+            out = run_loop()
             e.record()
         barrier()
     eager_launches = L.launch_count() - eager0      # launches outside the graph (hoisted garment passes, prepare)
@@ -554,6 +567,8 @@ def run_b200(args, rank, world, local):
     ms_per_step = total_ms / args.steps
     value = n_requests * args.steps / (total_ms / 1e3)
     log(f"timed region done: {ms_per_step:.1f} ms per bench step, {value:.3f} images/s")
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(args.dump_outputs, {"latents": out})
 
     # ---- rank 0: roofline inputs and the baselines (before the e2e section, so that a line can be printed even if the
     # e2e section does not come back)
@@ -596,14 +611,13 @@ def run_b200(args, rank, world, local):
                                        "region); try-on UNet per step from one CUDA graph"},
             "p50_latency_ms_per_image": statistics.median(per_step_ms) / len(groups),
             "latency_note": "latency of an image = loop time of the batch it belongs to",
-            # dominant kernel = the 2-CTA tcgen05 GEMM family (gemm2_kernel: ~60 % of the step in the ncu launch list,
-            # profiles/); timed live here on its largest launch shape with CUDA events, L2 flushed between launches,
-            # against the measured BURST bf16 peak (kernel timed alone). `step` = the whole timed loop against the
-            # SUSTAINED peak (algorithmic FLOPs of SURVEY.md App. B / device time).
+            # dominant kernel = the wgmma GEMM (the feed-forward GEMMs of the transformer blocks); timed live here on
+            # its largest launch shape with CUDA events, L2 flushed between launches, against the BURST bf16 peak
+            # (kernel timed alone). `step` = the whole timed loop against the SUSTAINED peak (algorithmic FLOPs of
+            # SURVEY.md App. B / device time).
             "roofline": {"bound": "tensor", "achieved": dom["tflops"], "peak": peaks["tflops_burst"], "unit": "TFLOP/s",
                          "frac": dom["tflops"] / peaks["tflops_burst"],
-                         "traffic": DOMINANT_KERNEL_DRAM_BYTES if dom.get("rows") == 3072 else None,   # ncu capture = config-2 shape
-                         "traffic_source": DOMINANT_KERNEL_TRAFFIC_SOURCE,
+                         "traffic": dom.get("bytes"), "traffic_source": "algorithmic bytes of the launch (A + W + out)",
                          "kernel": dom["kernel"], "algorithmic_flops_per_launch": dom["flops"],
                          "avg_launch_ms": dom["ms"], "launches_timed": dom["n"], "peak_source": peaks["source"],
                          "step": {"achieved": achieved, "peak": peaks["tflops"], "frac": achieved / peaks["tflops"],
@@ -687,7 +701,7 @@ def run_b200(args, rank, world, local):
             dt = tt.item()
         e2e = {"value": n_requests * n_e2e / dt, "unit": "images/s", "h2d_bytes_per_step": h2d * len(groups),
                "d2h_bytes_per_step": d2h * len(groups), "ms_per_call": dt / n_e2e / len(groups) * 1e3,
-               "includes": "H2D, VAE encodes (masked image, pose, cloth; fp32 NHWC engine route, fp16/TF32-operand tcgen05 convolutions), CLIP ViT-H image encoder "
+               "includes": "H2D, VAE encodes (masked image, pose, cloth; fp32 NHWC engine route, fp16/TF32-operand wgmma convolutions), CLIP ViT-H image encoder "
                "on the engine's kernels (uncond branch cached), Resampler, context K/V + hoisted garment passes, denoise loop, VAE decode, D2H of images"}
 
     guard_timer.cancel()
@@ -711,6 +725,9 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs (the latents of every batch of this "
+                         "rank, batch after batch) as DIR/<name>.npy (float32); engine arm only")
     ap.add_argument("--profile-one-step", action="store_true", help="run one denoise step inside a cudaProfiler range (ncu)")
     args = ap.parse_args()
     # watchdog: a bench that is still running after 20 minutes is stuck (the default run takes ~3 min) — dump every
@@ -718,6 +735,8 @@ def main():
     import faulthandler
     faulthandler.dump_traceback_later(int(os.environ.get("B200VTON_BENCH_WATCHDOG", "1200")), exit=True, file=sys.stderr)
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the engine's outputs; the reference arm (--impl reference) has none to write")
         rank = int(os.environ.get("RANK", "0"))
         run_reference(args, rank, int(os.environ.get("WORLD_SIZE", "1")))
         return

@@ -1,4 +1,4 @@
-"""idm-vton_b200 — Blackwell-native (sm_100a) engine for IDM-VTON's denoising hot path.
+"""idm-vton_b200 — Hopper-native (sm_90a) engine for IDM-VTON's denoising hot path.
 
 Import as `idm_vton_b200` (the root-level `idm_vton_b200.py` maps the importable name onto this directory).
 Layout: csrc/ (hand-written CUDA + C ABI), lib.py (ctypes binding), engine.py (UNet executors),

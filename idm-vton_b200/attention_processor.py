@@ -1,4 +1,4 @@
-"""Seam B3 (SURVEY.md 8b): the diffusers attention-processor protocol on the B200 kernels.
+"""Seam B3 (SURVEY.md 8b): the diffusers attention-processor protocol on the engine's kernels.
 
 Mirrors, name for name, the two processor classes the IDM-VTON inference path installs and the `Attention` container
 they are called with:
@@ -39,7 +39,7 @@ def _check_inputs(attn, hidden_states, attention_mask, who):
     if hidden_states.ndim != 3:
         raise NotImplementedError(f"{who}: expects token-major [B, T, C] hidden states")
     if not hidden_states.is_cuda or hidden_states.dtype != torch.float16:
-        raise RuntimeError(f"{who}: the B200 kernels need CUDA fp16 tensors (got {hidden_states.dtype} on "
+        raise RuntimeError(f"{who}: the engine's kernels need CUDA fp16 tensors (got {hidden_states.dtype} on "
                            f"{hidden_states.device}); there is no PyTorch fallback")
     if getattr(attn, "norm_cross", None):
         raise NotImplementedError(f"{who}: norm_cross is not on the IDM-VTON path")
@@ -178,7 +178,7 @@ class Attention(nn.Module):
         `to_out.0.{weight,bias}`) are registered afterwards under the reference's state-dict names."""
         super().__init__()
         if dim_head != 64 or bias:
-            raise NotImplementedError("the B200 attention kernels cover dim_head=64, bias-free q/k/v projections")
+            raise NotImplementedError("the engine's attention kernels cover dim_head=64, bias-free q/k/v projections")
         self.inner_dim = dim_head * heads
         self.cross_attention_dim = cross_attention_dim if cross_attention_dim is not None else query_dim
         self.heads = heads

@@ -1,4 +1,4 @@
-"""Builds libb200vton.so (hand-written sm_100a CUDA behind the C ABI of include/b200vton.h) in-tree with nvcc.
+"""Builds libb200vton.so (hand-written sm_90a CUDA behind the C ABI of include/b200vton.h) in-tree with nvcc.
 
 The shared object lives next to this file so it travels with the repo snapshot to the GPU box. Rebuilds only when a
 source is newer than the library.
@@ -10,10 +10,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200vton.so")
-SOURCES = ["host.cu", "gemm.cu", "gemm2.cu", "attn.cu", "attn6.cu", "attn_cross.cu", "attn_enc.cu", "conv_tf32.cu", "norm_f32.cu", "vae_f32.cu", "norm.cu", "elementwise.cu", "capi.cu"]
-HEADERS = ["common.cuh", "gemm_common.cuh", "host.h", os.path.join("..", "..", "include", "b200vton.h")]
+SOURCES = ["host.cu", "gemm.cu", "attn.cu", "norm_f32.cu", "vae_f32.cu", "norm.cu", "elementwise.cu", "capi.cu"]
+HEADERS = ["common.cuh", "gemm_common.cuh", "wgmma.cuh", "host.h", os.path.join("..", "..", "include", "b200vton.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -49,7 +49,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile every translation unit for sm_100a and link libb200vton.so. Returns the library path."""
+    """Compile every translation unit for sm_90a and link libb200vton.so. Returns the library path."""
     if not force and not needs_build():
         return LIB
     objdir = os.path.join(HERE, "build")
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(f"--- {s}\n{out}\n")
     if failed:
         raise RuntimeError("libb200vton build failed")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

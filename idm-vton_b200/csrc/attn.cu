@@ -1,45 +1,58 @@
-// Flash-style attention on tcgen05 for head_dim 64 with a TWO-SEGMENT key/value stream (sm_100a).
+// Flash-style attention on wgmma (sm_90a) for every attention of the project, one kernel:
 //
-// Replaces, on the try-on UNet's hot path (SURVEY.md 2.3 K9/K10):
 //   * attn1 of src/attentionhacked_tryon.py:334-348 + ip_adapter/attention_processor.py:238-262 — self-attention whose
 //     keys/values are [self tokens ; garment tokens]. Segment 0 = this sample's K/V, segment 1 = the cached garment K/V
 //     of sample (b - kv1_off) % kv1_count; the torch.cat never happens. Query rows are the N self tokens only
 //     (the reference computes and discards the Ng garment query rows).
 //   * CFG-uncond samples (b < kv1_off) see ZERO garment features (src/tryon_pipeline.py:1796): K=V=0, so each of the N1
 //     tokens adds exp(0 - m) to the softmax denominator and nothing to the numerator. Closed form, no KV traffic.
-//   * attn2 (ip_adapter/attention_processor.py:1943-1995): called twice (text tokens, then IP tokens with
-//     accumulate=1) — two independent softmaxes whose fp16 outputs are summed in fp16.
+//   * attn2 (ip_adapter/attention_processor.py:1943-1995, IPAttnProcessor2_0): the text softmax, then the IP-token softmax
+//     with accumulate = 1 and out_scale = ip_scale: out = fp16(fp16(O_t) + fp16(ip_scale * fp16(O_i))), the reference's
+//     rounding points (cross_attn_impl).
+//   * the CLIP towers' encoder self-attention (heads of 64 or 80, optional causal mask; enc_attn_impl).
 //
-// One CTA = one (sample, head, 128-query tile). Warp 0: TMA producer, warp 1: tcgen05.mma issuer, warps 2..5: softmax
-// (thread = query row). S = Q K^T lands in TMEM (fp32), softmax reads it with tcgen05.ld, writes P (fp16) into
-// 128B-swizzled smem, P V goes through the tensor core into a second TMEM tile that is folded into register
-// accumulators with the online-softmax rescale. Two CTAs are co-resident per SM so one CTA's softmax overlaps the other's MMAs.
+// Head dimension D = 16..96 in steps of 16: a head's columns are fetched as R = ceil(D/64) 128B-swizzled regions of 64
+// columns straight out of the projection buffer (the second region runs into the next head's columns, which are never
+// used: Q K^T issues exactly D/16 k-steps and the extra output columns of P V are never stored).
+//
+// One CTA = one (sample, head, 128-query tile): two warpgroups of 64 query rows each. Thread 0 issues the TMA loads (Q once,
+// K/V tiles of 128 keys through a 2-stage ring, the next tile of a stage as soon as both warpgroups have released it); a
+// separate producer warp would cap the consumers at 168 registers and make them spill. Per K/V tile a warpgroup computes
+// S = Q K^T (m64n128k16, both operands in shared memory) into registers, runs the online softmax there (a row lives in
+// the 4 threads of a quad), converts P to fp16 A fragments in registers and accumulates O += P V (m64nDNk16, V as the
+// MN-major B operand).
 #include "common.cuh"
 #include "host.h"
+#include "wgmma.cuh"
 
 namespace vton {
 
-struct AttnParams {
+struct FlashParams {
   __half* out;
   int ld_out;
   int B, H, Nq, N0, N1;
+  int D;          // head dimension: head h occupies columns [h*D, h*D + D)
   int kv1_off;    // segment-1 sample index = (b - kv1_off) % kv1_count; negative => zero K/V closed form
   int kv1_count;  // segment-1 sample index is taken modulo this count
   const int* kv1_base;  // optional device scalar added to the segment-1 sample index (hoisted per-step K/V)
+  int causal;     // key j visible to query i iff j <= i (segment 0 only)
   float scale_log2;
-  int accumulate;
+  int accumulate;   // out = old + fp16(out_scale * fp16(o)) instead of out = fp16(o)
+  float out_scale;
 };
 
-constexpr int AT_Q_BYTES = 128 * 128;      // 128 rows x 64 halves
-constexpr int AT_KV_BYTES = 128 * 128;     // one K or V tile
-constexpr int AT_P_BYTES = 2 * 128 * 128;  // 128 x 128 halves as two K-major regions
-constexpr int AT_STAGES = 2;
-constexpr int AT_OFF_Q = 0;
-constexpr int AT_OFF_K = AT_OFF_Q + AT_Q_BYTES;
-constexpr int AT_OFF_V = AT_OFF_K + AT_STAGES * AT_KV_BYTES;
-constexpr int AT_OFF_P = AT_OFF_V + AT_STAGES * AT_KV_BYTES;
-constexpr int AT_OFF_BAR = AT_OFF_P + AT_P_BYTES;
-constexpr int AT_SMEM_TOTAL = AT_OFF_BAR + 256 + 1024;
+constexpr int FA_REGION = 128 * 128;  // 128 rows x 64 halves
+constexpr int FA_STAGES = 2;
+constexpr int FA_THREADS = 256;       // 2 warpgroups; thread 0 also issues the TMA loads
+
+template <int R>
+struct FlashSmem {
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = OFF_Q + R * FA_REGION;
+  static constexpr int OFF_V = OFF_K + FA_STAGES * R * FA_REGION;
+  static constexpr int OFF_BAR = OFF_V + FA_STAGES * R * FA_REGION;
+  static constexpr int TOTAL = OFF_BAR + 64 + 1024;
+};
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -47,28 +60,45 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-__global__ void __launch_bounds__(192, 1)
-attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-            const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-            const __grid_constant__ CUtensorMap tmV1, const AttnParams p) {
+// KS: Q K^T k-steps (D / 16); R: 64-column regions per head; DN: P V tile width (64 for D <= 64, 96 otherwise)
+template <int KS, int R = (KS + 3) / 4, int DN = (KS <= 4 ? 64 : 96)>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
+             const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
+             const __grid_constant__ CUtensorMap tmV1, const FlashParams p) {
+  using SM = FlashSmem<R>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t bar_base = smem_base + AT_OFF_BAR;
+  const uint32_t bar_base = smem_base + SM::OFF_BAR;
   const uint32_t q_full = bar_base;
   auto kv_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bar_base + 8u * (1 + AT_STAGES + s); };
-  const uint32_t s_full = bar_base + 8u * (1 + 2 * AT_STAGES);
-  const uint32_t p_full = s_full + 8;
-  const uint32_t o_full = s_full + 16;
-  const uint32_t tmem_slot = s_full + 24;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_gen + AT_OFF_BAR + 8 * (4 + 2 * AT_STAGES));
+  auto kv_empty = [&](int s) { return bar_base + 8u * (1 + FA_STAGES + s); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int q_tile = blockIdx.x;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK0);
+    tma_prefetch_desc(&tmV0);
+    if (p.N1 > 0) {
+      tma_prefetch_desc(&tmK1);
+      tma_prefetch_desc(&tmV1);
+    }
+    mbar_init(q_full, 1);
+    for (int s = 0; s < FA_STAGES; ++s) {
+      mbar_init(kv_full(s), 1);
+      mbar_init(kv_empty(s), 2);   // one arrival per warpgroup
+    }
+    fence_barrier_init();
+  }
+  // Programmatic dependent launch: Q/K/V (and kv1_base) are written by the previous kernels of the stream
+  pdl_wait();
+  __syncthreads();
+  pdl_launch_dependents();
 
   const int tiles0 = (p.N0 + 127) >> 7;
   int idx1 = -1;
@@ -78,224 +108,230 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   }
   const bool zero_kv = (p.N1 > 0) && (idx1 < 0);
   const int tiles1 = (p.N1 > 0 && idx1 >= 0) ? ((p.N1 + 127) >> 7) : 0;
-  const int total = tiles0 + tiles1;
-  constexpr uint32_t kTmemCols = 256;
+  // causal: key tiles entirely after the last query row of this CTA contribute nothing
+  const int total = p.causal ? min(tiles0, q_tile + 1) : tiles0 + tiles1;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK0);
-    tma_prefetch_desc(&tmV0);
-    if (tiles1) {
-      tma_prefetch_desc(&tmK1);
-      tma_prefetch_desc(&tmV1);
-    }
-    mbar_init(q_full, 1);
-    for (int s = 0; s < AT_STAGES; ++s) {
-      mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 1);
-    mbar_init(o_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<kTmemCols>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  const uint32_t tmem_s = tmem_base;
-  const uint32_t tmem_pv = tmem_base + 128;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(q_full, AT_Q_BYTES);
-      tma_load_3d(smem_base + AT_OFF_Q, &tmQ, q_full, h * 64, q_tile * 128, b);
-      for (int j = 0; j < total; ++j) {
-        const int stage = j % AT_STAGES;
-        const uint32_t phase = (j / AT_STAGES) & 1;
-        mbar_wait(kv_empty(stage), phase ^ 1);
-        mbar_expect_tx(kv_full(stage), 2 * AT_KV_BYTES);
-        const uint32_t kdst = smem_base + AT_OFF_K + stage * AT_KV_BYTES;
-        const uint32_t vdst = smem_base + AT_OFF_V + stage * AT_KV_BYTES;
-        if (j < tiles0) {
-          tma_load_3d(kdst, &tmK0, kv_full(stage), h * 64, j * 128, b);
-          tma_load_3d(vdst, &tmV0, kv_full(stage), h * 64, j * 128, b);
-        } else {
-          tma_load_3d(kdst, &tmK1, kv_full(stage), h * 64, (j - tiles0) * 128, idx1);
-          tma_load_3d(vdst, &tmV1, kv_full(stage), h * 64, (j - tiles0) * 128, idx1);
-        }
+  // TMA loads are issued by thread 0: K/V tile j into stage j % FA_STAGES (the stage's previous tile must be released)
+  auto issue_kv = [&](int j) {
+    const int stage = j % FA_STAGES;
+    if (j >= FA_STAGES) mbar_wait(kv_empty(stage), ((j / FA_STAGES) - 1) & 1);
+    mbar_expect_tx(kv_full(stage), 2 * R * FA_REGION);
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const uint32_t kdst = smem_base + SM::OFF_K + (stage * R + r) * FA_REGION;
+      const uint32_t vdst = smem_base + SM::OFF_V + (stage * R + r) * FA_REGION;
+      const int col = h * p.D + r * 64;
+      if (j < tiles0) {
+        tma_load_3d(kdst, &tmK0, kv_full(stage), col, j * 128, b);
+        tma_load_3d(vdst, &tmV0, kv_full(stage), col, j * 128, b);
+      } else {
+        tma_load_3d(kdst, &tmK1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+        tma_load_3d(vdst, &tmV1, kv_full(stage), col, (j - tiles0) * 128, idx1);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_f16(128, 128, 0);  // S = Q K^T : B (keys x d) is K-major
-      constexpr uint32_t idesc_o = make_idesc_f16(128, 64, 1);   // O = P V   : B (d x keys) is MN-major
-      mbar_wait(q_full, 0);
-      for (int j = 0; j < total; ++j) {
-        const int stage = j % AT_STAGES;
-        const uint32_t phase = (j / AT_STAGES) & 1;
-        mbar_wait(kv_full(stage), phase);
-        tc_fence_after();
-        const uint32_t qsrc = smem_base + AT_OFF_Q;
-        const uint32_t ksrc = smem_base + AT_OFF_K + stage * AT_KV_BYTES;
-        const uint32_t vsrc = smem_base + AT_OFF_V + stage * AT_KV_BYTES;
+  };
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(q_full, R * FA_REGION);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          tc_mma_f16(tmem_s, make_smem_desc_sw128(qsrc + k * 32, 0, 1024), make_smem_desc_sw128(ksrc + k * 32, 0, 1024),
-                     idesc_s, k > 0 ? 1u : 0u);
-        }
-        tc_commit(s_full);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint32_t psrc = smem_base + AT_OFF_P;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t a_desc = make_smem_desc_sw128(psrc + (k >> 2) * 16384 + (k & 3) * 32, 0, 1024);
-          const uint64_t b_desc = make_smem_desc_sw128(vsrc + k * 2048, 16384, 1024);
-          tc_mma_f16(tmem_pv, a_desc, b_desc, idesc_o, k > 0 ? 1u : 0u);
-        }
-        tc_commit(kv_empty(stage));
-        tc_commit(o_full);
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const int q_idx = q_tile * 128 + row;
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    float m_run = -INFINITY, l_run = 0.f;
-    float o[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] = 0.f;
-    const float sl2 = p.scale_log2;
-    uint8_t* p_row = smem_gen + AT_OFF_P + row * 128;
-    const int rx = row & 7;
-
-    for (int j = 0; j < total; ++j) {
-      const int kv_valid = (j < tiles0) ? min(128, p.N0 - j * 128) : min(128, p.N1 - (j - tiles0) * 128);
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float s = (c * 32 + i < kv_valid) ? __uint_as_float(r[i]) : -INFINITY;
-          mx = fmaxf(mx, s);
-        }
-      }
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = fast_exp2((m_run - m_new) * sl2);
-      const float m_sc = m_new * sl2;
-      float sum = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = c * 32 + 2 * i;
-          const float p0 = (col < kv_valid) ? fast_exp2(__uint_as_float(r[2 * i]) * sl2 - m_sc) : 0.f;
-          const float p1 = (col + 1 < kv_valid) ? fast_exp2(__uint_as_float(r[2 * i + 1]) * sl2 - m_sc) : 0.f;
-          sum += p0 + p1;
-          pk[i] = pack_h2(p0, p1);
-        }
-        // 32 key columns = 4 chunks of 16 B inside region (c >> 1), 16B-chunk index ((c & 1) * 4 + q)
-        uint8_t* region = p_row + (c >> 1) * 16384;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int chunk = (c & 1) * 4 + q;
-          uint4 v = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-          *reinterpret_cast<uint4*>(region + ((chunk ^ rx) << 4)) = v;
-        }
-      }
-      l_run = l_run * alpha + sum;
-      m_run = m_new;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      named_bar_sync(1, 128);
-      if (threadIdx.x == 64) mbar_arrive(p_full);
-      mbar_wait(o_full, j & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_pv + lane_addr + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[c * 32 + i] = o[c * 32 + i] * alpha + __uint_as_float(r[i]);
-      }
-      tc_fence_before();
-    }
-    if (zero_kv) {
-      // N1 all-zero key/value tokens: score 0 each (App. D.3)
-      const float m_new = fmaxf(m_run, 0.f);
-      const float alpha = fast_exp2((m_run - m_new) * sl2);
-      l_run = l_run * alpha + static_cast<float>(p.N1) * fast_exp2(-m_new * sl2);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) o[i] *= alpha;
-    }
-    if (q_idx < p.Nq) {
-      const float inv = 1.f / l_run;
-      __half* dst = p.out + (static_cast<long long>(b) * p.Nq + q_idx) * p.ld_out + h * 64;
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        float v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = o[g * 8 + i] * inv;
-        if (p.accumulate) {
-          const uint4 old = *reinterpret_cast<const uint4*>(dst + g * 8);
-          const uint32_t ow[4] = {old.x, old.y, old.z, old.w};
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 a = unpack_h2(ow[i]);
-            v[2 * i] = a.x + round_h(v[2 * i]);
-            v[2 * i + 1] = a.y + round_h(v[2 * i + 1]);
-          }
-        }
-        uint4 ov;
-        ov.x = pack_h2(v[0], v[1]);
-        ov.y = pack_h2(v[2], v[3]);
-        ov.z = pack_h2(v[4], v[5]);
-        ov.w = pack_h2(v[6], v[7]);
-        *reinterpret_cast<uint4*>(dst + g * 8) = ov;
-      }
-    }
+    for (int r = 0; r < R; ++r)
+      tma_load_3d(smem_base + SM::OFF_Q + r * FA_REGION, &tmQ, q_full, h * p.D + r * 64, q_tile * 128, b);
+    for (int j = 0; j < FA_STAGES && j < total; ++j) issue_kv(j);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
+  // ===================== consumers =====================
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);   // this thread's rows: row0 and row0 + 8 of the tile
+  const int qi0 = q_tile * 128 + row0, qi1 = qi0 + 8;
+  const int cq = (lane & 3) * 2;                                 // first of this thread's two columns per 8-block
+  const float sl2 = p.scale_log2;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;    // l: this thread's partial row sums
+  float o[DN / 2];
+#pragma unroll
+  for (int i = 0; i < DN / 2; ++i) o[i] = 0.f;
+
+  mbar_wait(q_full, 0);
+  const uint32_t q_src = smem_base + SM::OFF_Q + wg * (64 * 128);
+  for (int j = 0; j < total; ++j) {
+    const int stage = j % FA_STAGES;
+    mbar_wait(kv_full(stage), (j / FA_STAGES) & 1);
+    const uint32_t k_src = smem_base + SM::OFF_K + stage * R * FA_REGION;
+    const uint32_t v_src = smem_base + SM::OFF_V + stage * R * FA_REGION;
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KS; ++k) {
+      const uint32_t off = (k >> 2) * FA_REGION + (k & 3) * 32;
+      WgmmaF16SS<128, 0>::mma(s, make_gmma_desc_sw128(q_src + off, 0, 1024), make_gmma_desc_sw128(k_src + off, 0, 1024),
+                              k > 0 ? 1 : 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+
+    const int key0 = (j < tiles0) ? j * 128 : (j - tiles0) * 128;
+    const int kv_valid = (j < tiles0) ? min(128, p.N0 - key0) : min(128, p.N1 - key0);
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int col = i * 8 + cq + u;
+        bool ok = col < kv_valid;
+        const bool ok0 = ok && (!p.causal || key0 + col <= qi0);
+        const bool ok1 = ok && (!p.causal || key0 + col <= qi1);
+        if (!ok0) s[4 * i + u] = -INFINITY;
+        if (!ok1) s[4 * i + 2 + u] = -INFINITY;
+        mx0 = fmaxf(mx0, s[4 * i + u]);
+        mx1 = fmaxf(mx1, s[4 * i + 2 + u]);
+      }
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    const float alpha0 = fast_exp2((m0 - mn0) * sl2), alpha1 = fast_exp2((m1 - mn1) * sl2);
+    const float ms0 = mn0 * sl2, ms1 = mn1 * sl2;
+    m0 = mn0;
+    m1 = mn1;
+    float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const float x0 = s[4 * i + u], x1 = s[4 * i + 2 + u];
+        const float p0 = x0 == -INFINITY ? 0.f : fast_exp2(x0 * sl2 - ms0);
+        const float p1 = x1 == -INFINITY ? 0.f : fast_exp2(x1 * sl2 - ms1);
+        s[4 * i + u] = p0;
+        s[4 * i + 2 + u] = p1;
+        sum0 += p0;
+        sum1 += p1;
+      }
+    }
+    l0 = l0 * alpha0 + sum0;
+    l1 = l1 * alpha1 + sum1;
+#pragma unroll
+    for (int i = 0; i < DN / 8; ++i) {
+      o[4 * i] *= alpha0;
+      o[4 * i + 1] *= alpha0;
+      o[4 * i + 2] *= alpha1;
+      o[4 * i + 3] *= alpha1;
+    }
+    // P (fp16, unnormalised, <= 1) as the A fragments of the 8 k-steps of 16 keys
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      pa[kk][0] = pack_h2(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_h2(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_h2(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_h2(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 V rows of 128 B per step
+      WgmmaF16RS<DN>::mma(o, pa[kk], make_gmma_desc_sw128(v_src + kk * 2048, FA_REGION, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty(stage));
+    if (threadIdx.x == 0 && j + FA_STAGES < total) issue_kv(j + FA_STAGES);
+  }
+
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  if (zero_kv) {
+    // N1 all-zero key/value tokens: score 0 each (App. D.3)
+    const float mn0 = fmaxf(m0, 0.f), mn1 = fmaxf(m1, 0.f);
+    const float alpha0 = fast_exp2((m0 - mn0) * sl2), alpha1 = fast_exp2((m1 - mn1) * sl2);
+    l0 = l0 * alpha0 + static_cast<float>(p.N1) * fast_exp2(-mn0 * sl2);
+    l1 = l1 * alpha1 + static_cast<float>(p.N1) * fast_exp2(-mn1 * sl2);
+#pragma unroll
+    for (int i = 0; i < DN / 8; ++i) {
+      o[4 * i] *= alpha0;
+      o[4 * i + 1] *= alpha0;
+      o[4 * i + 2] *= alpha1;
+      o[4 * i + 3] *= alpha1;
+    }
+  }
+  const float inv[2] = {1.f / l0, 1.f / l1};
+  const int qi[2] = {qi0, qi1};
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    if (qi[hr] >= p.Nq) continue;
+    __half* dst = p.out + (static_cast<long long>(b) * p.Nq + qi[hr]) * p.ld_out + h * p.D;
+#pragma unroll
+    for (int i = 0; i < DN / 8; ++i) {
+      const int col = i * 8 + cq;
+      if (col >= p.D) continue;
+      float v0 = o[4 * i + 2 * hr] * inv[hr], v1 = o[4 * i + 2 * hr + 1] * inv[hr];
+      if (p.accumulate) {
+        const float2 a = unpack_h2(*reinterpret_cast<const uint32_t*>(dst + col));
+        v0 = a.x + round_h(p.out_scale * round_h(v0));
+        v1 = a.y + round_h(p.out_scale * round_h(v1));
+      }
+      *reinterpret_cast<uint32_t*>(dst + col) = pack_h2(v0, v1);
+    }
   }
 }
 
-static int g_attn_v2 = 1;   // 1: attn6.cu (pipelined, P in tensor memory) for Nq >= 256; 0: this one-tile kernel always
-int attn6_launch(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
-                 const CUtensorMap& tmV1, __half* out, int ld_out, int B, int H, int Nq, int N0, int N1, int kv1_off,
-                 int kv1_count, const int* kv1_base, float scale_log2, int accumulate, int q_tiles, int poly,
-                 cudaStream_t stream);
-// attn6: exponentials (of every 4) evaluated by the FMA-pipe polynomial instead of the SFU. Measured on B200
-// (profiles/r1_attention_poly_exp.jsonl): 0 -> 695, 1 -> 683, 2 -> 573 TFLOP/s at the 3072-token level: the extra FMA-pipe
-// issue slots cost more than the SFU slots they free, so the default is 0.
-static int g_attn_poly = 0;
-void set_attn_poly(int n) { g_attn_poly = n; }
-static int g_attn_qtiles = 0;  // attn6: query tiles per CTA (0 = by K/V length, 1, 2)
-void set_attn_qtiles(int n) { g_attn_qtiles = n; }
-void set_attn_v2(int on) { g_attn_v2 = on; }
+// Tuning switches of other attention kernels of this library's C ABI; there is one attention kernel here, so the options
+// "attention_pingpong", "attention_q_tiles" and "attention_poly_exp" are accepted and have no effect.
+void set_attn_poly(int) {}
+void set_attn_qtiles(int) {}
+void set_attn_v2(int) {}
 
 static int encode_tokens(CUtensorMap* tm, const void* base, long long ld, int cols, int n, int batch) {
   uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(n), static_cast<uint64_t>(batch)};
   uint64_t strides[2] = {static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(n) * ld * 2};
   uint32_t box[3] = {64, 128, 1};
   return encode_tmap_f16(tm, base, 3, dims, strides, box);
+}
+
+template <int KS>
+static int launch_flash(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
+                        const CUtensorMap& tmV1, const FlashParams& p, cudaStream_t stream) {
+  constexpr int R = (KS + 3) / 4;
+  auto kern = flash_kernel<KS>;
+  static bool configured = false;
+  if (!configured) {
+    VTON_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FlashSmem<R>::TOTAL));
+    configured = true;
+  }
+  dim3 grid((p.Nq + 127) / 128, p.H, p.B);
+  VTON_CUDA(launch_kernel(kern, grid, dim3(FA_THREADS), FlashSmem<R>::TOTAL, stream, tmQ, tmK0, tmV0, tmK1, tmV1, p));
+  count_launch();
+  return kOk;
+}
+
+// One launch: q [B, Nq, >= H*D] (row stride ldq); k0/v0 [B, N0, .] (ldkv0); k1/v1 [B1, N1, .] (ldkv1) or null.
+static int flash(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+                 const void* v1, long long ldkv1, int B1, void* out, long long ldo, FlashParams p, cudaStream_t stream) {
+  CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
+  const int cols = p.H * p.D;
+  if (int e = encode_tokens(&tmQ, q, ldq, cols, p.Nq, p.B)) return e;
+  if (int e = encode_tokens(&tmK0, k0, ldkv0, cols, p.N0, p.B)) return e;
+  if (int e = encode_tokens(&tmV0, v0, ldkv0, cols, p.N0, p.B)) return e;
+  tmK1 = tmK0;
+  tmV1 = tmV0;
+  if (k1 != nullptr) {
+    if (int e = encode_tokens(&tmK1, k1, ldkv1, cols, p.N1, B1)) return e;
+    if (int e = encode_tokens(&tmV1, v1, ldkv1, cols, p.N1, B1)) return e;
+  }
+  p.out = static_cast<__half*>(out);
+  p.ld_out = static_cast<int>(ldo);
+  switch (p.D / 16) {
+    case 1: return launch_flash<1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+    case 2: return launch_flash<2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+    case 3: return launch_flash<3>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+    case 4: return launch_flash<4>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+    case 5: return launch_flash<5>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+    case 6: return launch_flash<6>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
+  }
+  set_last_error("attention: head dim %d unsupported", p.D);
+  return kErrUnsupported;
 }
 
 // q: [B, Nq, >=H*64] (row stride ldq); k0/v0: [B, N0, .] (ldkv0); k1/v1: [B1, N1, .] (ldkv1); out: [B, Nq, .] (ldo)
@@ -308,45 +344,74 @@ int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long
   const bool has1 = N1 > 0 && B1 > 0 && k1 && v1;
   VTON_CHECK_ARG(N1 == 0 || has1 || kv1_off >= B, "attn: segment 1 declared (N1=%d) but no K/V given", N1);
   VTON_CHECK_ARG(!has1 || ldkv1 % 8 == 0, "attn: ldkv1 must be a multiple of 8");
-  CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
-  if (int e = encode_tokens(&tmQ, q, ldq, H * 64, Nq, B)) return e;
-  if (int e = encode_tokens(&tmK0, k0, ldkv0, H * 64, N0, B)) return e;
-  if (int e = encode_tokens(&tmV0, v0, ldkv0, H * 64, N0, B)) return e;
-  tmK1 = tmK0;
-  tmV1 = tmV0;
-  if (has1) {
-    if (int e = encode_tokens(&tmK1, k1, ldkv1, H * 64, N1, B1)) return e;
-    if (int e = encode_tokens(&tmV1, v1, ldkv1, H * 64, N1, B1)) return e;
-  }
-  if (g_attn_v2 && Nq >= 256) {
-    return attn6_launch(tmQ, tmK0, tmV0, tmK1, tmV1, static_cast<__half*>(out), static_cast<int>(ldo), B, H, Nq, N0, N1,
-                          has1 ? kv1_off : (N1 > 0 ? B : 0), has1 ? (kv1_mod > 0 ? kv1_mod : B1) : 1,
-                          has1 ? static_cast<const int*>(kv1_base) : nullptr, scale * 1.4426950408889634f, accumulate,
-                          g_attn_qtiles, g_attn_poly, stream);
-  }
-  AttnParams p{};
-  p.out = static_cast<__half*>(out);
-  p.ld_out = static_cast<int>(ldo);
+  FlashParams p{};
   p.B = B;
   p.H = H;
   p.Nq = Nq;
   p.N0 = N0;
   p.N1 = N1;
+  p.D = 64;
   p.kv1_off = has1 ? kv1_off : (N1 > 0 ? B : 0);
   p.kv1_count = has1 ? (kv1_mod > 0 ? kv1_mod : B1) : 1;
   p.kv1_base = has1 ? static_cast<const int*>(kv1_base) : nullptr;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.accumulate = accumulate;
-  static bool configured = false;
-  if (!configured) {
-    VTON_CUDA(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM_TOTAL));
-    configured = true;
-  }
-  dim3 grid((Nq + 127) / 128, H, B);
-  attn_kernel<<<grid, 192, AT_SMEM_TOTAL, stream>>>(tmQ, tmK0, tmV0, tmK1, tmV1, p);
-  count_launch();
-  VTON_CUDA(cudaGetLastError());
-  return kOk;
+  p.out_scale = 1.f;
+  return flash(q, ldq, k0, v0, ldkv0, has1 ? k1 : nullptr, has1 ? v1 : nullptr, ldkv1, B1, out, ldo, p, stream);
+}
+
+// Decoupled cross-attention of the try-on / garment transformer blocks:
+//     out = fp16( fp16(softmax(Q Kt^T * scale) Vt) + fp16(ip_scale * fp16(softmax(Q Ki^T * scale) Vi)) )
+// Kt/Vt = the text tokens (attn2.to_k / to_v), Ki/Vi = the IP-Adapter image tokens (to_k_ip / to_v_ip); with Ni = 0 it is
+// the plain text cross-attention of the garment UNet (src/attentionhacked_garmnet.py:371-383).
+// q/out: [B, Nq, >= H*64]; kt/vt: [B, Nt, .] (row stride ldkv_t); ki/vi: [B, Ni, .] (ldkv_i) or null with Ni = 0
+int cross_attn_impl(const void* q, long long ldq, const void* kt, const void* vt, long long ldkv_t, int Nt,
+                    const void* ki, const void* vi, long long ldkv_i, int Ni, void* out, long long ldo, int B, int H,
+                    int Nq, float scale, float ip_scale, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && H > 0 && Nq > 0, "cross_attn: bad sizes B=%d H=%d Nq=%d", B, H, Nq);
+  VTON_CHECK_ARG(Nt > 0 && Nt <= 80 && Ni >= 0 && Ni <= 16, "cross_attn: needs 1 <= Nt <= 80 and Ni <= 16 (got %d, %d)", Nt, Ni);
+  VTON_CHECK_ARG(q && kt && vt && out && (Ni == 0 || (ki && vi)), "cross_attn: null pointer");
+  VTON_CHECK_ARG(ldq % 8 == 0 && ldkv_t % 8 == 0 && ldo % 8 == 0 && (Ni == 0 || ldkv_i % 8 == 0),
+                 "cross_attn: row strides must be multiples of 8");
+  VTON_CHECK_ARG(B <= 65535 && H <= 65535, "cross_attn: grid too large");
+  FlashParams p{};
+  p.B = B;
+  p.H = H;
+  p.Nq = Nq;
+  p.N0 = Nt;
+  p.D = 64;
+  p.kv1_count = 1;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out_scale = 1.f;
+  if (int e = flash(q, ldq, kt, vt, ldkv_t, nullptr, nullptr, 0, 0, out, ldo, p, stream)) return e;
+  if (Ni == 0) return kOk;
+  p.N0 = Ni;
+  p.accumulate = 1;
+  p.out_scale = ip_scale;
+  return flash(q, ldq, ki, vi, ldkv_i, nullptr, nullptr, 0, 0, out, ldo, p, stream);
+}
+
+// Encoder self-attention of the CLIP towers around the denoising loop: the ViT-H image encoder (16 heads of 80, 257
+// tokens) and the two text encoders (heads of 64, 77 tokens, causal mask).
+// q / k / v: [B, N, >= H*D] views (row strides ldq / ldkv, e.g. the three column blocks of a fused QKV buffer);
+// out: [B, N, H*D] (row stride ldo)
+int enc_attn_impl(const void* q, long long ldq, const void* k, const void* v, long long ldkv, void* out, long long ldo,
+                  int B, int H, int N, int D, float scale, int causal, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && H > 0 && N > 0, "encoder_attention: bad sizes B=%d H=%d N=%d", B, H, N);
+  VTON_CHECK_ARG(D >= 16 && D <= 96 && D % 16 == 0, "encoder_attention: head dim %d unsupported (16..96, multiple of 16)", D);
+  VTON_CHECK_ARG(ldq % 8 == 0 && ldkv % 8 == 0 && ldo % 8 == 0, "encoder_attention: row strides must be multiples of 8");
+  VTON_CHECK_ARG(B <= 65535 && H <= 65535, "encoder_attention: grid too large");
+  FlashParams p{};
+  p.B = B;
+  p.H = H;
+  p.Nq = N;
+  p.N0 = N;
+  p.D = D;
+  p.kv1_count = 1;
+  p.causal = causal ? 1 : 0;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out_scale = 1.f;
+  return flash(q, ldq, k, v, ldkv, nullptr, nullptr, 0, 0, out, ldo, p, stream);
 }
 
 }  // namespace vton

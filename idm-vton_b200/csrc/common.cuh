@@ -1,5 +1,5 @@
-// Shared device-side primitives for the sm_100a kernels of the IDM-VTON denoising engine:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and UMMA descriptors.
+// Shared device-side primitives for the sm_90a kernels of the IDM-VTON denoising engine:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and GMMA shared-memory descriptors.
 // Everything here is inline PTX; there is no CUTLASS on the include path.
 #pragma once
 #include <cuda.h>
@@ -10,7 +10,6 @@
 
 namespace vton {
 
-constexpr int kSMs = 148;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -48,17 +47,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug must trap instead of hanging the GPU (a hung box is a lost run).
+// Bounded wait: a pipeline bug must trap instead of hanging the GPU. No printf here: a call inside a loop that has
+// wgmma groups in flight makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
-  uint64_t t0 = globaltimer_ns();
+  const uint64_t t0 = globaltimer_ns();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 4000000000ull) {
-      printf("b200vton: mbarrier timeout block(%d,%d,%d) thread %d bar %u parity %u\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
   }
 }
 
@@ -104,168 +100,38 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp, same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrives (count 1) on the mbarrier when all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variants: a CTA pair in one cluster shares operands and issues one MMA of M = 256.
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> CTA 0's copy
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive (count 1) on the mbarrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(cta)
-      : "memory");
-}
-// TMA loads issued by either CTA of the pair; the transaction bytes are credited to CTA 0's mbarrier.
-__device__ __forceinline__ void tma2_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// Same, multicast: the box lands at the same CTA-relative smem offset of every CTA in cta_mask (cluster ranks) and
-// the bytes are credited to the barrier of each destination CTA's pair leader.
-__device__ __forceinline__ void tma2_load_2d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                                uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "h"(cta_mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
-                                             int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_dst, uint32_t cols) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// commit of the pair's MMAs: arrives on the mbarrier at this smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_2cta(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
 // Programmatic dependent launch: let the next kernel in the stream start its set-up now / wait until every kernel
 // this one depends on has completed and its memory is visible (no-ops when launched without the attribute).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// Instruction descriptor (cute::UMMA::InstrDescriptor bit layout): fp16 A/B, fp32 D, K-major A,
-// B K-major (b_mn_major = 0) or MN-major (1).
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t b_mn_major) {
-  return (1u << 4)                // c_format  = F32
-         | (0u << 7)              // a_format  = F16
-         | (0u << 10)             // b_format  = F16
-         | (0u << 15)             // a_major   = K
-         | (b_mn_major << 16)     // b_major
-         | ((N >> 3) << 17)       // n_dim
-         | ((M >> 4) << 24);      // m_dim
+// ----------------------------------------------------------------------------------------------
+// wgmma (warpgroup MMA): issue fence, group commit / wait, and the shared-memory matrix descriptor
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs that own the registers.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout), SWIZZLE_128B, version 1.
-//   K-major  operand, tile rows of 128 B (64 halves):   LBO ignored, SBO = 1024 B (8 rows x 128 B)
-//   MN-major operand, 64-wide MN atom (128 B rows along K): SBO = 1024 B (8 k-rows), LBO = MN-atom stride
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor (GMMA layout), SWIZZLE_128B; the tile base must be 1024-byte aligned.
+//   K-major  operand, rows of 128 B (64 halves / 32 floats): LBO unused, SBO = 1024 B (8 rows x 128 B)
+//   MN-major operand, 64-wide MN atom (128 B rows along K):   SBO = 1024 B (8 k-rows), LBO = MN-atom stride
+__device__ __forceinline__ uint64_t make_gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3ffff) >> 4);          // start address, bits [0,14)
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fff) << 16;  // leading byte offset, bits [16,30)
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fff) << 32;  // stride byte offset, bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                          // version = 1 (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                          // layout type = SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                          // layout type = SWIZZLE_128B
   return d;
 }
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns; thread t of warp w gets lane 32*(w%4)+t.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM, same lane/column mapping as tmem_ld_32x32
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

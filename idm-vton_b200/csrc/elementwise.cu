@@ -1,4 +1,4 @@
-// HBM-/latency-bound glue kernels of the denoise step (sm_100a): layout seams, samplers' data movement,
+// HBM-/latency-bound glue kernels of the denoise step (sm_90a): layout seams, samplers' data movement,
 // timestep embeddings, skinny (M <= 16) linears, and the fused CFG + DDPM update.
 // Reference call sites are cited per kernel; rounding points follow the fp16-autocast path (SURVEY.md App. D.1).
 #include "common.cuh"

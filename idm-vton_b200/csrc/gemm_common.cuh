@@ -1,5 +1,5 @@
-// Shared pieces of the tcgen05 GEMM / implicit-conv kernels (gemm.cu: 1-CTA tiles, gemm2.cu: 2-CTA persistent):
-// the problem descriptor, the accumulator-row -> output-row mapping and the fused epilogue.
+// Shared pieces of the wgmma GEMM / implicit-conv kernel (gemm.cu): the problem descriptor, the accumulator-row ->
+// output-row mapping and the fused epilogue.
 #pragma once
 #include "common.cuh"
 
@@ -30,6 +30,10 @@ struct GemmParams {
   int act_gelu;  // v = fp16(act(fp16(acc + bias))) before the later epilogue terms; 1 = erf-GELU (Resampler FeedForward, CLIP
                  // ViT-H / bigG MLPs), 2 = quick-GELU (CLIP ViT-L text MLP)
   int stride;    // conv: input pixel step per output pixel (1, or 2 = Downsample2D: the A map steps by 2 pixels per row)
+  // fp32-output convolution (the VAE): out = acc + bias (+ residual), all fp32; `out` above is unused then
+  float* out_f32;
+  const float* bias_f32;
+  const float* res_f32;
 };
 
 constexpr int BM = 128;
@@ -57,8 +61,7 @@ __device__ __forceinline__ void map_row(const GemmParams& p, int m_tile, int r_l
 }
 
 // Epilogue specialisation (compile time): which terms exist. EPI_RUNTIME keeps every term behind a runtime test of the
-// GemmParams pointers (1-CTA kernel, rare combinations); the others strip the unused code so the epilogue warps —
-// one per scheduler — execute ~100 instead of ~1000 instructions per 32-column chunk (ncu, profiles/r1_ncu_notes.md).
+// GemmParams pointers.
 enum : int { EPI_BIAS = 1, EPI_ROWVEC = 2, EPI_RES = 4, EPI_RUNTIME = 8 };
 
 // erf-GELU with the Abramowitz-Stegun 7.1.26 rational/exponential form (|abs err| < 2e-7, far below the fp16 rounding
@@ -79,15 +82,23 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   return 0.5f * x * (1.0f + erf_v);
 }
 
-// issue the TMEM loads of chunk c (no wait): accumulator 0 into acc, the gate half / shortcut accumulator into acc2
+// chunk c of one accumulator row from the fp32 staging tile in shared memory: accumulator 0 into acc, the gate half /
+// shortcut accumulator into acc2
 template <int BN, bool GEGLU, int EPI>
-__device__ __forceinline__ void epilogue_load(const GemmParams& p, uint32_t t_row, uint32_t sc_col_off, int c,
+__device__ __forceinline__ void epilogue_load(const GemmParams& p, const float* row, const float* row_sc, int c,
                                               uint32_t (&acc)[32], uint32_t (&acc2)[32]) {
-  tmem_ld_32x32(t_row + c * 32, acc);
-  if (GEGLU) {
-    tmem_ld_32x32(t_row + BN / 2 + c * 32, acc2);
-  } else if ((EPI & EPI_RUNTIME) && p.slabs_sc) {
-    tmem_ld_32x32(t_row + sc_col_off + c * 32, acc2);
+#pragma unroll
+  for (int i = 0; i < 32; i += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(row + c * 32 + i);
+    acc[i] = __float_as_uint(v.x), acc[i + 1] = __float_as_uint(v.y), acc[i + 2] = __float_as_uint(v.z), acc[i + 3] = __float_as_uint(v.w);
+  }
+  const float* src2 = GEGLU ? row + BN / 2 : (((EPI & EPI_RUNTIME) && p.slabs_sc) ? row_sc : nullptr);
+  if (src2 != nullptr) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(src2 + c * 32 + i);
+      acc2[i] = __float_as_uint(v.x), acc2[i + 1] = __float_as_uint(v.y), acc2[i + 2] = __float_as_uint(v.z), acc2[i + 3] = __float_as_uint(v.w);
+    }
   }
 }
 
@@ -207,29 +218,20 @@ __device__ __forceinline__ void epilogue_math(const GemmParams& p, int n_tile, l
   }
 }
 
-template <int BN, bool GEGLU, int EPI>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, uint32_t t_row, uint32_t sc_col_off, int n_tile,
-                                               long long out_row, int sample, int c, uint32_t (&pk)[16],
-                                               const uint4* res_pre = nullptr, const uint4* bias_pre = nullptr) {
-  uint32_t acc[32];
-  uint32_t acc2[32];
-  epilogue_load<BN, GEGLU, EPI>(p, t_row, sc_col_off, c, acc, acc2);
-  tmem_ld_wait();
-  epilogue_math<BN, GEGLU, EPI>(p, n_tile, out_row, sample, c, acc, acc2, pk, res_pre, bias_pre);
-}
-
-// Sink 1 (1-CTA kernel): registers -> global, each thread writes its own row.
+// Registers -> global, each thread writes the 32-column chunks c = c_first, c_first + c_step, ... of its own row.
 template <int BN, bool GEGLU>
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, uint32_t t_row, uint32_t sc_col_off, int n_tile,
-                                               long long out_row, int sample) {
+__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float* row, const float* row_sc, int n_tile,
+                                               long long out_row, int sample, int c_first, int c_step) {
   constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
   const int out_n0 = GEGLU ? n_tile * (BN / 2) : n_tile * BN;
   const int out_N = GEGLU ? p.N / 2 : p.N;
 #pragma unroll 1
-  for (int c = 0; c < OUT_COLS / 32; ++c) {
+  for (int c = c_first; c < OUT_COLS / 32; c += c_step) {
+    if (out_row < 0 || out_n0 + c * 32 >= out_N) continue;
+    uint32_t acc[32], acc2[32];
     uint32_t pk[16];
-    epilogue_chunk<BN, GEGLU, EPI_RUNTIME>(p, t_row, sc_col_off, n_tile, out_row, sample, c, pk);
-    if (out_row < 0) continue;
+    epilogue_load<BN, GEGLU, EPI_RUNTIME>(p, row, row_sc, c, acc, acc2);
+    epilogue_math<BN, GEGLU, EPI_RUNTIME>(p, n_tile, out_row, sample, c, acc, acc2, pk);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       const int ncol = out_n0 + c * 32 + g * 8;

@@ -18,10 +18,20 @@ void set_last_error(const char* fmt, ...) {
 }
 const char* get_last_error() { return g_err; }
 
-// Off by default for eager launches, switched on by denoise.py for the kernel nodes of the captured step graph. Round 1 saw
-// two stalls with it on every launch: a dependent CTA held all tensor memory while it waited for a primary that had not
-// allocated yet. The kernels now wait BEFORE tcgen05.alloc; re-validated on B200 in round 2 (4 of 4 bench runs with PDL on
-// every launch clean, compute-sanitizer synccheck / memcheck clean: profiles/r2_compute_sanitizer.md, r2_pdl_in_graph.json).
+// Off by default for eager launches, switched on by denoise.py for the kernel nodes of the captured step graph. Every kernel
+// launched with the attribute calls griddepcontrol.wait before it reads global memory written by its predecessors.
+int num_sms() {
+  static std::atomic<int> cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
+
 static std::atomic<int> g_pdl{0};
 int pdl_enabled() { return g_pdl.load(std::memory_order_relaxed); }
 void set_pdl(int on) { g_pdl.store(on ? 1 : 0, std::memory_order_relaxed); }

@@ -44,9 +44,12 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
+// Streaming multiprocessors of the current device (read once per device: 132 on an H100 SXM, fewer on other parts).
+int num_sms();
+
 // Programmatic dependent launch (option "programmatic_launch", default OFF, see host.cu): the hot kernels are launched
 // with cudaLaunchAttributeProgrammaticStreamSerialization; they initialise their barriers and prefetch tensor maps, call
-// griddepcontrol.wait, only then allocate tensor memory and touch global memory, and call
+// griddepcontrol.wait, only then touch global memory, and call
 // griddepcontrol.launch_dependents once they hold all their resources — so the launch latency and part of the set-up
 // of kernel n+1 overlap the tail of kernel n (~930 launches per captured denoise step).
 int pdl_enabled();

@@ -1,4 +1,4 @@
-// GroupNorm(32) (+SiLU) and LayerNorm for the UNets' NHWC / token-major fp16 activations (sm_100a, HBM-bound).
+// GroupNorm(32) (+SiLU) and LayerNorm for the UNets' NHWC / token-major fp16 activations (sm_90a, HBM-bound).
 //
 // Reference rounding points (SURVEY.md App. D.1): under torch.cuda.amp.autocast the norms run in fp32 on the fp16
 // input and return fp32; SiLU stays fp32; the consuming conv / linear casts to fp16. So both kernels compute in fp32
@@ -283,7 +283,8 @@ int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW
   const int ws_rows = B > 296 ? B : 296;
   GnBarrier* bar = reinterpret_cast<GnBarrier*>(partial + static_cast<long long>(ws_rows) * 64);
   // RESIDENT: one CTA per SM, its rows parked in shared memory
-  int chunks_r = kSMs / B;
+  int chunks_r = num_sms() / B;
+  if (chunks_r * B > ws_rows) chunks_r = ws_rows / B;   // the partial-sum workspace holds ws_rows (sample, chunk) rows
   if (chunks_r > cdiv(HW, 16)) chunks_r = cdiv(HW, 16);
   bool resident = false;
   int rows_per_cta = 0, chunks = 0;
@@ -295,7 +296,8 @@ int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW
     }
   }
   if (!resident) {
-    chunks = (kSMs * occ_stream) / B;   // every CTA of the launch co-resident
+    chunks = (num_sms() * occ_stream) / B;   // every CTA of the launch co-resident
+    if (chunks * B > ws_rows) chunks = ws_rows / B;
     if (chunks < 1) chunks = 1;         // B > capacity: one CTA per sample, nobody waits for anybody
     if (chunks > cdiv(HW, 16)) chunks = cdiv(HW, 16);
     rows_per_cta = cdiv(HW, chunks);

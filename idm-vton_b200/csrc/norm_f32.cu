@@ -3,8 +3,7 @@
 // src/tryon_pipeline.py:913-915,1076-1093). Same structure as the fp16 kernels of norm.cu — deterministic two-stage
 // statistics (per-(sample, chunk, group) partial sums in double, no atomics), then one normalise(+SiLU) pass — with
 // fp32 in/out and float4 accesses; HBM-bound: 3 * B*HW*C*4 bytes per call (up to 2.4 GB at 1024x768x128).
-// Validated on B200 in round 2 (tests/test_kernels_gpu.py -k "fp32_nhwc or vae_nhwc", profiles/r2_vae_nhwc.json) and ON by
-// default in the VAE's NHWC route (idm-vton_b200/vae.py).
+// Checked by tests/test_kernels_gpu.py -k "fp32_nhwc or vae_nhwc"; ON by default in the VAE's NHWC route (idm-vton_b200/vae.py).
 #include "common.cuh"
 #include "host.h"
 

@@ -2,7 +2,7 @@
 // of 512 channels over H*W tokens, exact fp32 in the reference because src/tryon_pipeline.py:913-915,1076-1093 upcasts the
 // VAE). idm-vton_b200/vae.py runs its products on the TF32 tensor cores three times with split operands
 // (a.b ~ a_lo.b_hi + a_hi.b_lo + a_hi.b_hi); these kernels produce the split operands in ONE pass each instead of the five
-// ATen passes per split that profiles/r2_vae_kernel_shares.json shows (the probabilities alone are 100 MB per 2048-query chunk
+// ATen passes per split (the probabilities alone are 100 MB per 2048-query chunk
 // and image):
 //   split_tf32:          x (* scale) -> hi = tf32(x), lo = tf32(x - hi), both exactly representable in TF32, so the tensor
 //                        core (which ignores the 13 low mantissa bits of its fp32 operands) sees them unchanged;
@@ -43,7 +43,7 @@ int split_tf32_impl(const void* x, long long stride_b, int B, long long per_batc
                      (reinterpret_cast<uintptr_t>(lo) & 15) == 0, "split_tf32: pointers must be 16-byte aligned");
   const long long total4 = static_cast<long long>(B) * per_batch / 4;
   long long blocks = (total4 + 255) / 256;
-  if (blocks > kSMs * 16) blocks = kSMs * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   split_tf32_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(static_cast<const float*>(x), stride_b, per_batch, scale,
                                                                       static_cast<float*>(hi), static_cast<float*>(lo), total4);
   count_launch();

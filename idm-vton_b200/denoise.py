@@ -1,4 +1,4 @@
-"""The denoising hot loop of IDM-VTON on the B200 engine (src/tryon_pipeline.py:1765-1866).
+"""The denoising hot loop of IDM-VTON on the engine (src/tryon_pipeline.py:1765-1866).
 
 Per step the reference runs the garment UNet (batch Bg), zero-pads its 70 features for the CFG-uncond half, runs the
 try-on UNet (batch 2B), applies CFG and the DDPM update. Here one step is a fixed launch sequence over static buffers:
@@ -64,9 +64,9 @@ class GarmentKVCache:
     """LRU cache of hoisted garment K/V across requests (SURVEY.md 8f item 4). One entry = the K/V of ONE garment for every
     denoise step and every try-on block ([T, Ng, 2C] fp16 per block: 4.7 GB at 768x1024 / 30 steps), keyed by the caller's
     garment id plus everything the values depend on (timestep list, latent size). A hit replaces the garment's T
-    garment-UNet passes (~160 ms per garment on B200) by device-to-device copies (~2 ms)."""
+    garment-UNet passes by device-to-device copies (~2 ms)."""
 
-    def __init__(self, max_bytes=40 << 30):
+    def __init__(self, max_bytes=16 << 30):   # beside 11 GB of weights and the step's K/V on an 80 GB H100
         import collections
         self.max_bytes = int(max_bytes)
         self.entries = collections.OrderedDict()
@@ -224,9 +224,8 @@ class TryOnDenoiser:
 
     @property
     def garment_chunk(self):
-        """Timesteps batched into one hoisted garment-UNet pass. Measured on B200 at config 2 (2 garments): 8 -> 1096 ms per
-        loop, 15 -> 1085, 30 -> 1081 (fewer, larger launches: 936 instead of 3708 eager launches per loop); default = up to
-        64 samples per pass."""
+        """Timesteps batched into one hoisted garment-UNet pass (fewer, larger launches); default = up to 64 samples
+        per pass."""
         if self._garment_chunk:
             return self._garment_chunk
         return max(1, 64 // max(1, getattr(self, "Bg", 1)))
@@ -292,13 +291,10 @@ class TryOnDenoiser:
         self.latents.copy_(self.latents_next)
 
     # Programmatic dependent launch INSIDE the captured step only (B200VTON_PDL_GRAPH, default below): every kernel node
-    # of the graph is one of this library's kernels, which call griddepcontrol.wait before they allocate tensor memory
-    # or touch global memory, so the set-up of kernel n+1 overlaps the tail of kernel n (+1.3 % of the loop, round 1).
-    # Eager launches — which interleave with cuBLAS / cuDNN / ATen kernels in the pipeline call, where round 1 saw two
-    # stalls before the wait-before-alloc fix — keep plain stream order unless B200VTON_PDL=1 asks otherwise.
-    # Round 2 on B200: 1126 -> 1116 ms per 30-step loop (profiles/r2_pdl_in_graph.json), 3 of 3 bench runs with the e2e
-    # section clean; with PDL on every launch (eager ones included) 4 of 4 clean after the wait-before-alloc fix and
-    # `compute-sanitizer --tool synccheck` reports no hazard. Default: ON inside the graph, OFF for eager launches.
+    # of the graph is one of this library's kernels, which call griddepcontrol.wait before they touch global
+    # memory, so the set-up of kernel n+1 overlaps the tail of kernel n. Eager launches, which interleave with cuBLAS /
+    # cuDNN / ATen kernels in the pipeline call, keep plain stream order unless B200VTON_PDL=1 asks otherwise.
+    # Default: ON inside the graph, OFF for eager launches.
     PDL_IN_GRAPH = __import__("os").environ.get("B200VTON_PDL_GRAPH", "1") == "1"
 
     def capture(self):

@@ -340,7 +340,7 @@ class UNetEngine:
         h = L.gemm(a2.view(B * N, C), blk.wo2, bias=blk.bo2, residual=h)
         n3 = L.layernorm(h, blk.ln3w, blk.ln3b)
         ff = L.gemm(n3, blk.wff1, bias=blk.bff1, geglu=True,
-                    force_bn=(1000 + blk.ff_bn) if n3.shape[0] >= 512 else blk.ff_bn)   # 2-CTA kernel for large M
+                    force_bn=blk.ff_bn)   # the tile width the GEGLU weights were packed for
         return L.gemm(ff, blk.wff2, bias=blk.bff2, residual=h)
 
     def _t2d(self, t, x, state):

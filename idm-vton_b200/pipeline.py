@@ -3,7 +3,7 @@
 Same constructor components, `encode_prompt` and `__call__` signatures and defaults as src/tryon_pipeline.py:387-401,
 511-526,1254-1301 (tests/test_pipeline_signature.py compares them with `ast`), same call-time behaviour
 (check_inputs errors, RNG draw order, CFG ordering [uncond ; cond], `(images,)` tuple return, the
-`output_type="latent"` quirk), but the denoising loop (:1765-1866) runs on the B200 engine:
+`output_type="latent"` quirk), but the denoising loop (:1765-1866) runs on the engine:
 both UNets, garment-feature attention, CFG and the DDPM update are libb200vton.so launches replayed from one CUDA
 graph per step (denoise.TryOnDenoiser). Pre/post-processing (VAE, CLIP) is host-side PyTorch plumbing.
 """
@@ -366,7 +366,7 @@ class StableDiffusionXLInpaintPipeline:
                                  f" got: `prompt_embeds` {prompt_embeds.shape} != `negative_prompt_embeds`"
                                  f" {negative_prompt_embeds.shape}.")
         if padding_mask_crop is not None:
-            raise ValueError("padding_mask_crop is not supported by the B200 engine pipeline (not used by inference.py)")
+            raise ValueError("padding_mask_crop is not supported by the engine pipeline (not used by inference.py)")
 
     def _fused_preprocess_ok(self, image, mask_image, height, width):
         """The one-launch pre-processing covers what inference.py passes: CUDA float tensors [B,3,H,W] / [B,1|3,H,W]
@@ -716,7 +716,7 @@ class StableDiffusionXLInpaintPipeline:
 
         if trace:
             trace.mark("clip_image_encoder+resampler")
-        # 11. denoising loop on the B200 engine
+        # 11. denoising loop on the engine
         self._num_timesteps = len(timesteps)
         # unet.engine() re-packs after load_state_dict() / .to() on the module; a denoiser built on older engines (and its
         # captured graph) would silently run stale weights

@@ -302,7 +302,7 @@ class _UNetBase(nn.Module):
             lib.load()
             self._lib = lib
         if self.device.type != "cuda" or self.dtype != torch.float16:
-            raise RuntimeError("the B200 engine needs the UNet on a CUDA device in fp16 "
+            raise RuntimeError("the engine needs the UNet on a CUDA device in fp16 "
                                f"(got {self.device}, {self.dtype}); there is no CPU / PyTorch fallback")
 
     def engine(self):
@@ -339,7 +339,7 @@ class _UNetBase(nn.Module):
             proc = processor.pop(name) if isinstance(processor, dict) else processor
             want = IPAttnProcessor2_0 if (ip and name.endswith("attn2.processor")) else AttnProcessor2_0
             if type(proc) is not want:
-                raise TypeError(f"{name}: the B200 engine fuses {want.__name__} here (got {type(proc).__name__}); other "
+                raise TypeError(f"{name}: the engine fuses {want.__name__} here (got {type(proc).__name__}); other "
                                 "processors have no kernel and there is no PyTorch fallback")
             if want is IPAttnProcessor2_0:
                 exp = (attn.to_q.weight.shape[0], attn.to_k.weight.shape[1])

@@ -5,7 +5,7 @@ The reference pipeline receives a diffusers `AutoencoderKL` as a component (src/
 force_upcast,latent_channels,block_out_channels}` (:911-932,1646,1868-1880). diffusers is not installable in this image, so
 this module supplies an architecture-compatible VAE (same parameter names as diffusers 0.25.0's AutoencoderKL, restated
 from its published structure) so that `__call__` runs end to end. The VAE is row (f)1 of SURVEY.md 8 ("next"): on a GPU
-the fp32 VAE runs NHWC with its 3x3 / stride-1 convolutions on the tcgen05 kernels `b200vton_conv3x3_nhwc_f32` (TF32
+the fp32 VAE runs NHWC with its 3x3 / stride-1 convolutions on the wgmma kernels `b200vton_conv3x3_nhwc_f32` (TF32
 operands) / `b200vton_conv3x3_nhwc_f16in_f32` (fp16 operands handed over by the norm: `_gn_silu_conv`) and every GroupNorm(+SiLU)
 on `b200vton_groupnorm_nhwc_f32` (default ON, see `_ENGINE_NHWC`), the resnets' residual add rides in the convolution's epilogue, the mid-block attention is a split-TF32 formulation (cuBLAS GEMMs between this library's one-pass split /
 softmax kernels); resampling and the stride-2 / 3-8-channel / 1x1 convolutions are PyTorch.
@@ -19,15 +19,12 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 
-# Measured on B200 (profiles/r1_vae_tf32_conv.jsonl): the kernel beats cuDNN on every VAE convolution shape (478-809 vs
-# 349-643 TFLOP/s), but the VAE as a whole got SLOWER (encode 78 vs 63 ms, decode 138 vs 107 ms per 2 images): the
-# convolutions are only ~15% of its time, the rest is fp32 GroupNorm / SiLU / resampling / attention passes over up to
-# 805 MB tensors, and feeding an NHWC kernel from torch's NCHW GroupNorm adds two layout copies per convolution. The
-# switch therefore stays off until those passes have NHWC kernels of their own (B200VTON_VAE_TF32_CONV=1 to enable).
+# Feeding the NHWC convolution from torch's NCHW GroupNorm adds two layout copies per convolution over tensors of up to
+# 805 MB, while the convolutions are a minor part of the VAE's time; this NCHW switch therefore stays off
+# (B200VTON_VAE_TF32_CONV=1 to enable) and the NHWC route below is the engine's path.
 _ENGINE_CONV = os.environ.get("B200VTON_VAE_TF32_CONV", "0") == "1"
 # The whole fp32 VAE in NHWC (channels_last): the engine convolution then needs no layout copies and GroupNorm(+SiLU) runs on
-# `b200vton_groupnorm_nhwc_f32`. Validated on B200 in round 2 (tests -k "fp32_nhwc or vae_nhwc"; profiles/r2_vae_nhwc.json):
-# encode 62.5 -> 30.1 ms, decode 106.5 -> 50.6 ms per 2 images at 1024x768 (fp16 cuDNN: 46 / 82 ms). Default ON
+# `b200vton_groupnorm_nhwc_f32` (checked by tests -k "fp32_nhwc or vae_nhwc"). Default ON
 # (B200VTON_VAE_NHWC=0 restores the cuDNN NCHW route); fp32 data, TF32 products — the arithmetic class the reference's
 # fp32 VAE gets from cuDNN under torch's default `cudnn.allow_tf32`.
 _ENGINE_NHWC = os.environ.get("B200VTON_VAE_NHWC", "1") == "1"
@@ -135,15 +132,14 @@ def _split_tf32(x):
 def _attention_fp32_3xtf32(q, k, v, chunk=2048):
     """softmax(q k^T / sqrt(C)) v for the VAE mid block — ONE head of C = 512 channels over H*W tokens (12288 at
     768x1024), exact fp32 in the reference (SDPA on fp32 tensors with torch's default matmul precision). PyTorch's fp32
-    memory-efficient kernel spends 11.3 ms per batch-2 pass on B200 (no tensor cores). Here every product runs on the TF32
+    memory-efficient kernel uses no tensor cores. Here every product runs on the TF32
     tensor cores three times with split operands — a·b ≈ a_hi·b_hi + a_hi·b_lo + a_lo·b_hi, fp32 accumulation — which
     removes the TF32 operand rounding (the dropped a_lo·b_lo term is 2^-22 relative); what remains is the tensor core's own
     fp32 accumulation over thousands of keys: 3.9e-5 max abs error against fp64 at 3072 keys where fp32 SDPA has 3.6e-6
     and a single TF32 pass 3.0e-3 (tests/test_kernels_gpu.py) — an order below the error of the TF32 convolutions around
     it. Queries are processed in chunks so the score block stays small. The products are cuBLAS TF32 GEMMs; the split operands and
     the softmax come from `b200vton_split_tf32` / `b200vton_softmax_split_tf32` (one pass each; the three score products are ONE
-    GEMM over the concatenated contraction [q_lo | q_hi | q_hi] . [k_hi | k_lo | k_hi]^T, small terms first), which took the
-    VAE from 125.2 to 110.7 ms per (6-image encode + 2-image decode) on B200; `_ATTN_FUSED = False` is the ATen formulation
+    GEMM over the concatenated contraction [q_lo | q_hi | q_hi] . [k_hi | k_lo | k_hi]^T, small terms first); `_ATTN_FUSED = False` is the ATen formulation
     of the same arithmetic (kept as the cross-check of tests/test_kernels_gpu.py). Host-side plumbing of a SURVEY 8f row."""
     B, N, C = q.shape
     prev = torch.backends.cuda.matmul.allow_tf32
@@ -339,8 +335,6 @@ class AutoencoderKL(nn.Module):
         return types.SimpleNamespace(latent_dist=dist) if return_dict else (dist,)
 
     def decode(self, z, return_dict=True, generator=None):
-        # (cuDNN's channels_last kernels and its autotuner were both measured on B200 for these fp32 convolutions:
-        # channels_last is slower — encode 221 vs 173 ms, decode 150 vs 113 ms per call — and autotuning changes nothing)
         if _use_nhwc(z):
             img = self.decoder(self.post_quant_conv(z.contiguous(memory_format=torch.channels_last))).contiguous()
         else:

@@ -1,4 +1,4 @@
-/* libb200vton.so — C ABI of the Blackwell-native IDM-VTON denoising engine.
+/* libb200vton.so — C ABI of the Hopper-native (sm_90a) IDM-VTON denoising engine.
  *
  * The reference (yisol/IDM-VTON) has no C/FFI plugin API; its seams are Python protocols (SURVEY.md 8b: pipeline
  * __call__, UNet2DConditionModel.forward, the diffusers attention-processor protocol). This header is the boundary the
@@ -27,18 +27,11 @@ int b200vton_version(void);
 const char* b200vton_last_error(void);
 /* kernels launched (or recorded into a capturing stream) by this library since it was loaded */
 long long b200vton_launch_count(void);
-/* library options: "gemm_2cta_auto" = 1 (default) lets gemm / conv3x3 pick the 2-CTA persistent kernel for large
- * problems when force_bn == 0; 0 keeps every launch on the 1-CTA kernel. "attention_pingpong" = 1 (default) runs
- * b200vton_attention on the pipelined kernel (attn6.cu: S issued one tile ahead, P in tensor memory) when Nq >= 256;
- * 0 keeps the one-tile kernel (attn.cu), which the tests use as an independent cross-check.
- * ("attention_q_tiles" = 1 | 2 pins the pipelined kernel's query tiles per CTA, 0 = chosen from the K/V length;
- * "attention_poly_exp" = 0 | 1 | 2 of every 4 exponentials evaluated by an FMA-pipe polynomial instead of the SFU,
- * default 0: measured slower).
- * "gemm_cluster4" = 1 runs large linear layers with 256-wide tiles in four-CTA clusters whose CTA pairs multicast the
- * shared A slabs; 0 (default: it measured slower on B200) keeps two-CTA clusters.
- * "programmatic_launch" = 1 launches the hot kernels with programmatic stream serialization (their set-up overlaps
- * the previous kernel's tail; they wait for it before allocating tensor memory or touching global memory);
- * 0 (default) = plain stream order. */
+/* library options: "programmatic_launch" = 1 launches the hot kernels with programmatic stream serialization (their
+ * set-up overlaps the previous kernel's tail; they wait for it before touching global memory); 0 (default) = plain
+ * stream order. "gemm_2cta_auto", "gemm_cluster4", "attention_pingpong", "attention_q_tiles" and "attention_poly_exp"
+ * select kernel variants of other GPU generations; they are accepted and have no effect (one GEMM and one attention
+ * kernel on sm_90a). */
 int b200vton_set_option(const char* name, int value);
 
 /* out[M,N] = epi(A[M,K] . W[N,K]^T): nn.Linear on the hot path — attn to_q/to_k/to_v/to_out
@@ -50,8 +43,8 @@ int b200vton_set_option(const char* name, int value);
  * flags & 2 (GELU): v = fp16(gelu_erf(fp16(acc + bias))) before the rowvec / residual terms (ip_adapter/resampler.py:13-20;
  *             the CLIP ViT-H / bigG MLPs). flags & 4 (quick-GELU): v = fp16(x * sigmoid(1.702 x)), x = fp16(acc + bias)
  *             (the CLIP ViT-L text encoder's MLP, src/tryon_pipeline.py:592).
- * K % 64 == 0; N, lda, ldw, ldo % 8 == 0. force_bn: 0 = automatic kernel and tile width; 64/128/160/256 = 1-CTA
- * kernel with that tile width; 1000 + {128,160,192,256} = 2-CTA persistent kernel (cta_group::2) with that width. */
+ * K % 64 == 0; N, lda, ldw, ldo % 8 == 0. force_bn: 0 = automatic tile width; 64/128/160/256 = that tile width;
+ * 1000 + width and 2000 + width select the same width (encodings of multi-CTA variants). */
 int b200vton_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, void* out, int64_t ldo, int M, int N,
                       int K, const void* bias, const void* residual, int64_t ldr, const void* rowvec,
                       int64_t ld_rowvec, int rows_per_sample, int flags, int force_bn, void* stream);
@@ -62,7 +55,7 @@ int b200vton_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, vo
  * output pixel (TMA traversal stride), so no im2col buffer exists.
  * x: [B,H,W,Cin] with channel stride ldx; w: [9][Cout][Cin] (tap = ky*3+kx); out: [B*Ho*Wo, ldo], Ho = (H-1)/stride+1.
  * epi: v = fp16(acc + bias); v = fp16(v + temb[b, n]) (time_emb_proj broadcast add);
- *      1x1 shortcut (w_sc [Cout, C0+C1] over the channel concat of sc0|sc1, accumulated in a second TMEM tile):
+ *      1x1 shortcut (w_sc [Cout, C0+C1] over the channel concat of sc0|sc1, accumulated in a second register accumulator):
  *      s = fp16(acc_sc + bias_sc); v = fp16(s + v);   identity residual: v = fp16(v + residual[m, n]). */
 int b200vton_conv3x3_nhwc(const void* x, int64_t ldx, int B, int H, int W, int Cin, const void* w, int Cout,
                           const void* bias, const void* temb, int64_t ld_temb, const void* sc0, int C0,

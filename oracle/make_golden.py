@@ -1,6 +1,6 @@
 """Pins oracle/unet_ref.py against the REFERENCE's own modules and writes tests/golden/*.pt.
 
-Runs only in the build container (needs /root/reference). The reference's src/*.py and ip_adapter/*.py are imported
+Needs a checkout of the original project (IDM_VTON_REFERENCE). The reference's src/*.py and ip_adapter/*.py are imported
 UNMODIFIED and in place, on top of the test-only diffusers shim (oracle/shim), with seeded synthetic weights generated
 by oracle.unet_ref.make_state_dict (loaded with strict=True: this also pins the state-dict key names / shapes).
 
@@ -12,13 +12,13 @@ import sys
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("IDM_VTON_REFERENCE", "")   # checkout of the original IDM-VTON project
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def import_reference():
     if not os.path.isdir(REF):
-        raise RuntimeError("/root/reference is not available: golden fixtures can only be regenerated in the build container")
+        raise RuntimeError("set IDM_VTON_REFERENCE to a checkout of the original project to regenerate the golden fixtures")
     sys.path.insert(0, os.path.join(ROOT, "oracle", "shim"))
     sys.path.insert(0, REF)
     import src.unet_hacked_tryon as ut  # noqa: E402

@@ -1,7 +1,7 @@
 """Golden vectors of the REFERENCE pipeline `StableDiffusionXLInpaintPipeline.__call__` (src/tryon_pipeline.py:1254-1896)
 at BASELINE config 1 (256x256 px, 2 denoise steps, batch 1, CPU fp32).
 
-Runs only in the build container (needs /root/reference). `src/tryon_pipeline.py`, `src/unet_hacked_tryon.py`,
+Needs a checkout of the original project (IDM_VTON_REFERENCE). `src/tryon_pipeline.py`, `src/unet_hacked_tryon.py`,
 `src/unet_hacked_garmnet.py` and `ip_adapter/*.py` are imported UNMODIFIED and in place on the diffusers shim; the
 components diffusers / the HF hub would supply (not available offline) are stand-ins with seeded weights:
   unet / unet_encoder   the reference's own UNet2DConditionModel classes, tiny SDXL-topology config (oracle.unet_ref.tiny_config)
@@ -23,7 +23,7 @@ import sys
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("IDM_VTON_REFERENCE", "")   # checkout of the original IDM-VTON project
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 H = W = 256
 STEPS = 2

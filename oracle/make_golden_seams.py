@@ -1,6 +1,6 @@
 """Golden vectors for the seam tests (tests/test_seams_gpu.py), produced by the REFERENCE's own code.
 
-Runs only in the build container (needs /root/reference). Imported unmodified and in place:
+Needs a checkout of the original project (IDM_VTON_REFERENCE). Imported unmodified and in place:
   * ip_adapter/attention_processor.py  AttnProcessor2_0 (:189-278), IPAttnProcessor2_0 (:1879-2010), executed on the
     diffusers-shim `Attention` container (oracle/shim/diffusers/models/attention_processor.py), CPU fp32;
   * ip_adapter/resampler.py            Resampler at the geometry the try-on UNet hard-codes
@@ -17,7 +17,7 @@ import sys
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("IDM_VTON_REFERENCE", "")   # checkout of the original IDM-VTON project
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 

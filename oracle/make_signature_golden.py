@@ -1,11 +1,11 @@
 """Extracts the reference pipeline's public signatures with `ast` (no import of the reference needed) and writes
-tests/golden/pipeline_signature.json. Runs only where /root/reference exists."""
+tests/golden/pipeline_signature.json. Needs a checkout of the original project (IDM_VTON_REFERENCE)."""
 import ast
 import json
 import os
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = "/root/reference/src/tryon_pipeline.py"
+SRC = os.path.join(os.environ.get("IDM_VTON_REFERENCE", ""), "src", "tryon_pipeline.py")
 
 
 def signature(fn):

@@ -1,7 +1,7 @@
 """diffusers.image_processor for the shim: the reference pipeline only needs `VaeImageProcessor.preprocess/postprocess`
 (src/tryon_pipeline.py:418-421,1588-1602,1885). diffusers is not installable here, so the restatement that ships with
 the product (idm-vton_b200/vae.py, host-side plumbing) serves both sides; its semantics are "parity unpinned"
-(no diffusers source under /root/reference)."""
+(no diffusers source under the reference)."""
 import os
 import sys
 

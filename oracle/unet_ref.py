@@ -3,7 +3,7 @@
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this module.
 Nothing here is used by the product path (idm-vton_b200/), which must fail loudly when libb200vton.so is missing.
 
-What it restates (reference file:line, relative to /root/reference):
+What it restates (reference file:line, relative to the reference):
   * try-on UNet forward            src/unet_hacked_tryon.py:1006-1395
   * garment UNet forward           src/unet_hacked_garmnet.py:917-1284   (returns the 70 garment features only)
   * block sequencing / skip cat    src/unet_block_hacked_tryon.py:724-781,1123-1201,1256-1289,2308-2397,2450-2507
@@ -14,13 +14,13 @@ What it restates (reference file:line, relative to /root/reference):
   * IPAttnProcessor2_0             ip_adapter/attention_processor.py:1907-2010 (decoupled text / IP softmax, scale 1.0)
   * Resampler / PerceiverAttention ip_adapter/resampler.py:49-78,164-176
 and, from the third-party dependency diffusers==0.25.0 (pinned environment.yaml:20, NOT vendored under
-/root/reference — restated from its published semantics, SURVEY.md App. C): ResnetBlock2D, Downsample2D, Upsample2D,
+the reference — restated from its published semantics, SURVEY.md App. C): ResnetBlock2D, Downsample2D, Upsample2D,
 Attention (weights only), GEGLU, Timesteps, TimestepEmbedding.
 
 Pinning: oracle/make_golden.py runs the reference's own src/*.py + ip_adapter/*.py IN PLACE on the diffusers shim
 (oracle/shim) with the same random weights and compares against this file (tests/test_oracle_pin.py re-checks the
 committed fixtures). The in-repo logic is therefore pinned to the reference; the diffusers leaf ops are "parity
-unpinned" (no upstream source, golden vectors or tests for them exist in /root/reference).
+unpinned" (no upstream source, golden vectors or tests for them exist in the reference).
 
 All functions are written with torch.nn.functional calls so that they run (i) on CPU in fp32 — the yard-stick and the
 timed CPU baseline — and (ii) on CUDA under torch.autocast(fp16) with fp16 weights, which reproduces the reference's

@@ -1,5 +1,5 @@
-"""Tile-width (BN) sweep of the 2-CTA GEMM / conv kernel on the shapes where the round-1 divisibility rule and the round-2
-cost model (gemm.cu pick_bn2) disagree, with cuBLAS beside it. Tuning aid; prints JSON lines."""
+"""Tile-width (BN) sweep of the GEMM / conv kernel (forced widths vs the automatic choice of gemm.cu pick_bn) on the UNet's
+shapes, with cuBLAS beside it. Tuning aid; prints JSON lines."""
 import json
 import os
 import sys

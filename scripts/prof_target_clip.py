@@ -1,4 +1,4 @@
-"""ncu target: the CLIP ViT-H self-attention launch (B=2, 16 heads of 80, 257 tokens) and the bigG text one (B=2, 20 heads of
+"""Profiler target (torch.cuda.profiler range): the CLIP ViT-H self-attention launch (B=2, 16 heads of 80, 257 tokens) and the bigG text one (B=2, 20 heads of
 64, 77 tokens, causal), a few times each."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""ncu launch-list target: one fp32 VAE encoder pass of 6 images (masked image, pose, garment of a config-2 batch) and one
+"""Profiler target (torch.cuda.profiler range): one fp32 VAE encoder pass of 6 images (masked image, pose, garment of a config-2 batch) and one
 decoder pass of 2 latents at 1024x768, after one warm-up of each (profiler range around the measured passes)."""
 import os
 import sys

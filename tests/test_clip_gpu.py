@@ -2,7 +2,7 @@
 
 The reference calls `transformers` modules here (src/tryon_pipeline.py:468-470, 592-612); `transformers` is importable on
 the GPU box, so the checker is the module itself: fp32 (TF32 off) = truth, fp16 = the reference's execution mode
-(inference.py:268-274 loads the encoders with torch_dtype=float16). Contract as for the UNets (DESIGN.md section 3): the
+(inference.py:268-274 loads the encoders with torch_dtype=float16). Contract as for the UNets (tests/test_fullsize_gpu.py): the
 engine must not be further from the fp32 truth than the fp16 module is (+ slack), metric max|a-b| / max(1, max|b|).
 """
 import math
@@ -72,7 +72,7 @@ def test_encoder_attention_peaky_and_scale():
 def test_gemm_quick_gelu_epilogue():
     from idm_vton_b200 import lib as L
     g = torch.Generator(device="cuda").manual_seed(1)
-    for M in (154, 1024):      # 1-CTA kernel / 2-CTA persistent kernel
+    for M in (154, 1024):      # one and several 128-row tiles
         a = torch.randn(M, 768, generator=g, device="cuda").half()
         w = (torch.randn(3072, 768, generator=g, device="cuda") * 0.05).half()
         b = torch.randn(3072, generator=g, device="cuda").half()

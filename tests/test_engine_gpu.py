@@ -1,4 +1,4 @@
-"""Parity of the B200 engine (both UNets + the denoise loop) against the oracle (oracle/unet_ref.py, loop_ref.py).
+"""Parity of the engine (both UNets + the denoise loop) against the oracle (oracle/unet_ref.py, loop_ref.py).
 
 Three yard-sticks, same seeded inputs / weights (fp16-rounded so every path sees identical values):
   * `ref32`  : oracle in fp32 on the GPU (TF32 off)            — the high-precision answer

@@ -327,7 +327,7 @@ def test_cfg_ddpm_step(lib):
 
 
 # ------------------------------------------------------------------------------------------------
-# 2-CTA persistent kernel (gemm2.cu): force_bn = 1000 + tile width
+# force_bn = 1000 + tile width: the C ABI's encoding of a forced width (64/128/160/192/256 of the one GEMM kernel)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("M,N,K,bn", [(256, 256, 64, 256), (512, 512, 128, 256), (3072, 1280, 1280, 256),
                                       (12288, 1920, 640, 192), (12288, 640, 640, 160), (1000, 640, 192, 128),
@@ -372,7 +372,7 @@ def test_conv3x3_2cta(lib, B, H, W, Cin, Cout, bn):
 
 
 def test_gemm_auto_matches_1cta(lib):
-    """Automatic kernel choice (2-CTA for large problems) gives the same fp16 results as the 1-CTA kernel."""
+    """The automatic tile-width choice gives the same fp16 results as a forced 256-wide tile."""
     a, w = rnd(4096, 1280, seed=1), rnd(1280, 1280, scale=1280 ** -0.5, seed=2)
     o_auto = lib.gemm(a, w)
     o_v1 = lib.gemm(a, w, force_bn=256)
@@ -380,7 +380,7 @@ def test_gemm_auto_matches_1cta(lib):
 
 
 # ------------------------------------------------------------------------------------------------
-# ping-pong attention kernel (attn2.cu, Nq >= 256) — the earlier attention tests with Nq >= 256 also run on it
+# attention at UNet sizes (Nq >= 256): two segments, ragged tails, the zero-K/V closed form
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("B,H,Nq,N0,Ng", [(1, 1, 256, 128, 0), (2, 5, 3072, 3072, 3072), (2, 3, 300, 500, 77),
                                           (2, 20, 768, 768, 768), (1, 2, 1024, 77, 0), (1, 2, 257, 16, 0)])
@@ -398,7 +398,8 @@ def test_attention_pingpong(lib, B, H, Nq, N0, Ng):
 
 
 def test_attention_pingpong_lazy_rescale(lib):
-    """Row maxima that grow by far more than 2^8 between K/V tiles force the TMEM rescale path."""
+    """Row maxima that grow by far more than 2^8 between K/V tiles exercise the online-softmax rescale of O. The
+    option attention_pingpong selects a kernel of another GPU generation; here it is accepted and changes nothing."""
     B, H, N = 1, 2, 512
     C = H * 64
     q = rnd(B, N, C, scale=3.0, seed=1)
@@ -412,7 +413,7 @@ def test_attention_pingpong_lazy_rescale(lib):
         out1 = lib.attention(q, k, v, heads=H)
     finally:
         lib.set_option("attention_pingpong", 1)
-    close(out, out1, tol=4e-3)
+    assert torch.equal(out, out1)
 
 
 def test_attention_per_step_kv_base(lib):
@@ -432,9 +433,9 @@ def test_attention_per_step_kv_base(lib):
 
 
 def test_attention_p_in_tmem_variant(lib):
-    """attn6.cu (P in its own tensor-memory columns, S issued one tile ahead, fp32 softmax) vs the one-tile kernel of
-    attn.cu (option attention_pingpong=0) and the fp32 reference: two segments with ragged tails, the zero-KV half, the
-    accumulate mode and a peaky distribution."""
+    """The attention kernel vs the fp32 reference: two segments with ragged tails, the zero-KV half, the accumulate mode
+    and a peaky distribution. The options attention_pingpong / attention_q_tiles select kernels of another GPU
+    generation; they are accepted and must not change the result."""
     Bp, H, N, Ng = 2, 5, 640, 1000
     C = H * 64
     qkv = rnd(2 * Bp, N, 3 * C, seed=21)
@@ -450,8 +451,8 @@ def test_attention_p_in_tmem_variant(lib):
     ref_u = _attn_ref(q[:Bp], k[:Bp], v[:Bp], H, 0.125, n_zero=Ng)
     close(o5[Bp:], ref_c, tol=3e-3)
     close(o5[:Bp], ref_u, tol=3e-3)
-    close(o5, o3, tol=2e-3)
-    for qt in (1, 2):   # one query tile per CTA (two CTAs per SM) / two query tiles sharing each K/V tile
+    assert torch.equal(o5, o3)
+    for qt in (1, 2):
         lib.set_option("attention_q_tiles", qt)
         try:
             oq = lib.attention(q, k, v, gkv[..., :C], gkv[..., C:], kv1_off=Bp, heads=H)
@@ -459,10 +460,9 @@ def test_attention_p_in_tmem_variant(lib):
             o9 = lib.attention(q9, k9, v9, heads=2)
         finally:
             lib.set_option("attention_q_tiles", 0)
-        close(oq[Bp:], ref_c, tol=3e-3)
-        close(oq[:Bp], ref_u, tol=3e-3)
+        assert torch.equal(oq, o5)
         close(o9, _attn_ref(q9, k9, v9, 2, 0.125), tol=4e-3)
-    # peaky scores exercise the lazy rescale of O in tensor memory; long single segment exercises the stage ring wrap
+    # peaky scores exercise the rescale of O; a long single segment exercises the K/V stage ring wrap
     q2, k2, v2 = rnd(1, 2048, 128, scale=4.0, seed=23), rnd(1, 2048, 128, seed=24), rnd(1, 2048, 128, seed=25)
     close(lib.attention(q2, k2, v2, heads=2), _attn_ref(q2, k2, v2, 2, 0.125), tol=4e-3)
     # accumulate mode (decoupled cross-attention adds the second attention onto the first)
@@ -476,8 +476,8 @@ def test_attention_p_in_tmem_variant(lib):
 @pytest.mark.parametrize("B,H,N,Nt,Ni", [(2, 10, 256, 77, 16), (4, 20, 768, 77, 16), (2, 10, 3072, 77, 0),
                                          (1, 5, 200, 77, 16), (3, 2, 40, 33, 7), (2, 4, 128, 80, 16)])
 def test_cross_attention_fused(lib, B, H, N, Nt, Ni):
-    """attn_cross.cu: text + IP-token cross-attention in one launch vs the fp32 reference with the reference's fp16
-    rounding points (two softmaxes, fp16 outputs summed in fp16) and vs the two-launch accumulate path."""
+    """cross_attention: text + IP-token cross-attention vs the fp32 reference with the reference's fp16 rounding points
+    (two softmaxes, fp16 outputs summed in fp16) and vs the two-call accumulate path."""
     C = H * 64
     q = rnd(B, N, 3 * C, seed=1)[..., C:2 * C]              # strided view, like a slice of a fused projection
     kvt = rnd(B, Nt, 2 * C, seed=2)
@@ -506,13 +506,13 @@ def test_cross_attention_ip_scale_and_peaky(lib):
     close(out, ref, tol=3e-3)
 
 
-@pytest.mark.parametrize("B,H,W,C0,C1,Cout,force_bn", [(2, 32, 24, 640, 320, 640, 1160), (2, 32, 24, 640, 320, 640, 1128),
-                                                      (4, 32, 24, 1280, 1280, 1280, 1256), (1, 32, 24, 320, 0, 640, 0),
+@pytest.mark.parametrize("B,H,W,C0,C1,Cout,force_bn", [(2, 32, 24, 640, 320, 640, 1064), (2, 32, 24, 640, 320, 640, 1128),
+                                                      (4, 32, 24, 1280, 1280, 1280, 64), (1, 32, 24, 320, 0, 640, 0),
                                                       (3, 16, 24, 1280, 640, 1280, 0), (2, 64, 48, 640, 320, 320, 0)])
 def test_conv3x3_shortcut_2cta_variants(lib, B, H, W, C0, C1, Cout, force_bn):
-    """Resnet conv2 with the fused 1x1 shortcut on the 2-CTA kernel (second TMEM accumulator, one accumulator stage):
-    against the fp32 reference with the reference's rounding (both conv outputs rounded to fp16, then added) and
-    against the 1-CTA kernel."""
+    """Resnet conv2 with the fused 1x1 shortcut (second register accumulator) at the tile widths a shortcut can use
+    (64 / 128, forced or automatic): against the fp32 reference with the reference's rounding (both conv outputs rounded
+    to fp16, then added) and against the 128-wide tile. A wider forced tile is refused with an error."""
     from idm_vton_b200.engine import pack_conv3x3
     h = rnd(B, H, W, Cout, seed=1)
     s0 = rnd(B, H, W, C0, seed=2)
@@ -527,11 +527,13 @@ def test_conv3x3_shortcut_2cta_variants(lib, B, H, W, C0, C1, Cout, force_bn):
     close(out, ref)
     v1 = lib.conv3x3(h, wp, bias=b2, sc0=s0, sc1=s1, w_sc=wsc, bias_sc=bsc, force_bn=128)
     close(out, v1, tol=1e-3)
+    with pytest.raises(RuntimeError, match="unsupported"):
+        lib.conv3x3(h, wp, bias=b2, sc0=s0, sc1=s1, w_sc=wsc, bias_sc=bsc, force_bn=1256)
 
 
 def test_gemm_four_cta_cluster_variant(lib):
-    """force_bn = 2256: the 2-CTA kernel in four-CTA clusters with multicast A slabs (off by default: measured slower).
-    Must be bit-identical to the two-CTA-cluster launch, including odd N-tile counts and ragged M."""
+    """force_bn = 2000 + width, the C ABI's encoding of a multicast-cluster variant, selects the same tile as 1000 + width:
+    bit-identical results (odd N-tile counts, ragged M, GEGLU) and the fp32 reference."""
     from idm_vton_b200.engine import pack_geglu
     for (M, N, K) in [(1024, 1280, 256), (3000, 768, 192), (2048, 512, 1280)]:
         a, w, b, r = rnd(M, K, seed=1), rnd(N, K, scale=K ** -0.5, seed=2), rnd(N, seed=3), rnd(M, N, seed=4)
@@ -545,8 +547,9 @@ def test_gemm_four_cta_cluster_variant(lib):
 
 
 def test_attention_polynomial_exp_fraction(lib):
-    """attn6.cu evaluates 0, 1 or 2 of every 4 exponentials with the FMA-pipe polynomial (default 0): all three against
-    the fp32 reference on a diffuse and on a peaky distribution with a ragged two-segment K/V stream."""
+    """The option attention_poly_exp (0, 1 or 2 polynomial exponentials of every 4 in a kernel of another GPU generation)
+    is accepted and has no effect: every setting is bit-identical and within tolerance of the fp32 reference on a diffuse
+    and on a peaky distribution with a ragged two-segment K/V stream."""
     Bp, H, N, Ng = 1, 3, 520, 700
     C = H * 64
     for qscale in (1.0, 5.0):
@@ -560,6 +563,9 @@ def test_attention_polynomial_exp_fraction(lib):
                 lib.set_option("attention_poly_exp", n)
                 o = lib.attention(q, k, v, gk, gv, kv1_off=Bp, heads=H)
                 errs.append((close(o[Bp:], ref_c, tol=3e-3), close(o[:Bp], ref_u, tol=3e-3)))
+                if n == 0:
+                    o0 = o
+                assert torch.equal(o, o0)
         finally:
             lib.set_option("attention_poly_exp", 0)
         print(f"qscale {qscale}: errors (cond, uncond) for poly 0/1/2: {errs}")
@@ -744,9 +750,8 @@ def test_vae_attention_fused_equals_aten_formulation(monkeypatch):
 
 
 def test_vae_attention_3xtf32_matches_fp32_sdpa():
-    """The VAE mid-block attention on split TF32 products (vae._attention_fp32_3xtf32) vs fp64 truth. Measured on B200 at
-    3072 keys: 3.9e-5 max abs error, against 3.6e-6 for PyTorch's fp32 SDPA (the reference's arithmetic) and 3.0e-3 for a
-    single TF32 pass: the split removes the operand rounding (75x), what remains is the tensor core's fp32 accumulation
+    """The VAE mid-block attention on split TF32 products (vae._attention_fp32_3xtf32) vs fp64 truth at 3072 keys,
+    beside PyTorch's fp32 SDPA (the reference's arithmetic) and a single TF32 pass: the split removes the operand rounding (75x), what remains is the tensor core's fp32 accumulation
     over thousands of keys (not IEEE round-to-nearest) — an order of magnitude below the error of the TF32 convolutions
     around it (6e-4 of scale, same file), which the reference's cuDNN path has too."""
     from idm_vton_b200.vae import _attention_fp32_3xtf32

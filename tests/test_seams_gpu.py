@@ -1,5 +1,5 @@
 """GPU parity of the drop-in seams (SURVEY.md 8b) against outputs of the REFERENCE's own code (tests/golden/*.pt, made by
-oracle/make_golden.py and oracle/make_golden_seams.py with /root/reference imported in place):
+oracle/make_golden.py and oracle/make_golden_seams.py with the reference imported in place):
 
   B3  attention-processor protocol : AttnProcessor2_0 / IPAttnProcessor2_0 (ip_adapter/attention_processor.py:189-278,
       1879-2010) called as `processor(attn, hidden_states, encoder_hidden_states, ...)`; `set_attn_processor`
@@ -190,7 +190,7 @@ def test_resampler_tiny_vs_reference_golden(tiny_modules):
 
 def test_resampler_sdxl_geometry_vs_reference_golden():
     """The Resampler at the geometry the try-on UNet hard-codes (src/unet_hacked_tryon.py:476-485) vs the output of
-    /root/reference/ip_adapter/resampler.py (loaded standalone by oracle/make_golden_seams.py)."""
+    the reference's ip_adapter/resampler.py (loaded standalone by oracle/make_golden_seams.py)."""
     from oracle.make_golden_seams import resampler_weights
     from idm_vton_b200 import lib as L
     from idm_vton_b200.unet import resampler_forward
