@@ -340,6 +340,7 @@ int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long
               int kv1_off, int kv1_mod, const void* kv1_base, float scale, int accumulate, cudaStream_t stream) {
   VTON_CHECK_ARG(B > 0 && H > 0 && Nq > 0 && N0 > 0 && N1 >= 0, "attn: bad sizes B=%d H=%d Nq=%d N0=%d N1=%d", B, H, Nq, N0, N1);
   VTON_CHECK_ARG(ldq % 8 == 0 && ldkv0 % 8 == 0 && ldo % 8 == 0, "attn: row strides must be multiples of 8");
+  VTON_CHECK_ARG(aligned_to(out, 4), "attn: out must be 4-byte aligned (stored two halves at a time)");
   VTON_CHECK_ARG(B <= 65535 && H <= 65535, "attn: grid too large");
   const bool has1 = N1 > 0 && B1 > 0 && k1 && v1;
   VTON_CHECK_ARG(N1 == 0 || has1 || kv1_off >= B, "attn: segment 1 declared (N1=%d) but no K/V given", N1);
@@ -373,6 +374,7 @@ int cross_attn_impl(const void* q, long long ldq, const void* kt, const void* vt
   VTON_CHECK_ARG(q && kt && vt && out && (Ni == 0 || (ki && vi)), "cross_attn: null pointer");
   VTON_CHECK_ARG(ldq % 8 == 0 && ldkv_t % 8 == 0 && ldo % 8 == 0 && (Ni == 0 || ldkv_i % 8 == 0),
                  "cross_attn: row strides must be multiples of 8");
+  VTON_CHECK_ARG(aligned_to(out, 4), "cross_attn: out must be 4-byte aligned (stored two halves at a time)");
   VTON_CHECK_ARG(B <= 65535 && H <= 65535, "cross_attn: grid too large");
   FlashParams p{};
   p.B = B;
@@ -400,6 +402,7 @@ int enc_attn_impl(const void* q, long long ldq, const void* k, const void* v, lo
   VTON_CHECK_ARG(B > 0 && H > 0 && N > 0, "encoder_attention: bad sizes B=%d H=%d N=%d", B, H, N);
   VTON_CHECK_ARG(D >= 16 && D <= 96 && D % 16 == 0, "encoder_attention: head dim %d unsupported (16..96, multiple of 16)", D);
   VTON_CHECK_ARG(ldq % 8 == 0 && ldkv % 8 == 0 && ldo % 8 == 0, "encoder_attention: row strides must be multiples of 8");
+  VTON_CHECK_ARG(aligned_to(out, 4), "encoder_attention: out must be 4-byte aligned (stored two halves at a time)");
   VTON_CHECK_ARG(B <= 65535 && H <= 65535, "encoder_attention: grid too large");
   FlashParams p{};
   p.B = B;

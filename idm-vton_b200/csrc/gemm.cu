@@ -299,6 +299,11 @@ int gemm_f16_impl(const void* A, long long lda, const void* W, long long ldw, vo
   VTON_CHECK_ARG(K % 64 == 0, "gemm: K=%d must be a multiple of 64", K);
   VTON_CHECK_ARG(N % 8 == 0 && lda % 8 == 0 && ldw % 8 == 0 && ldo % 8 == 0, "gemm: N/lda/ldw/ldo must be multiples of 8");
   VTON_CHECK_ARG(!geglu || (N % 16 == 0 && !residual && !rowvec), "gemm: bad GEGLU configuration");
+  // the epilogue reads bias / residual / rowvec and writes out 8 halves (16 bytes) at a time
+  VTON_CHECK_ARG(aligned_to(out, 16) && aligned_to(bias, 16) && aligned_to(residual, 16) && aligned_to(rowvec, 16),
+                 "gemm: out/bias/residual/rowvec must be 16-byte aligned");
+  VTON_CHECK_ARG((!residual || ldr % 8 == 0) && (!rowvec || ld_rowvec % 8 == 0),
+                 "gemm: ldr=%lld / ld_rowvec=%lld must be multiples of 8", ldr, ld_rowvec);
   const int bn = pick_bn(N, cdiv(M, BM), geglu != 0, false, force_bn);
   VTON_CHECK_ARG(bn != 0, "gemm: tile width force_bn=%d unsupported for this problem (N=%d, geglu=%d)", force_bn, N, geglu);
   VTON_CHECK_ARG(!geglu || N % bn == 0, "gemm: GEGLU needs N %% BN == 0 (N=%d, BN=%d)", N, bn);
@@ -370,6 +375,12 @@ int conv3x3_impl(const void* x, long long ldx, int B, int Hin, int Win, int Cin,
   VTON_CHECK_ARG(Cout % 8 == 0 && ldo % 8 == 0 && ldx % 8 == 0, "conv3x3: Cout/ldo/ldx must be multiples of 8");
   VTON_CHECK_ARG(C0 % 64 == 0 && C1 % 64 == 0, "conv3x3: shortcut source channels must be multiples of 64");
   VTON_CHECK_ARG(!(w_sc && residual), "conv3x3: shortcut conv and identity residual are exclusive");
+  // the epilogue reads bias / temb / bias_sc / residual and writes out 8 halves (16 bytes) at a time
+  VTON_CHECK_ARG(aligned_to(out, 16) && aligned_to(bias, 16) && aligned_to(temb, 16) && aligned_to(bias_sc, 16) &&
+                     aligned_to(residual, 16),
+                 "conv3x3: out/bias/temb/bias_sc/residual must be 16-byte aligned");
+  VTON_CHECK_ARG((!residual || ldr % 8 == 0) && (!temb || ld_temb % 8 == 0),
+                 "conv3x3: ldr=%lld / ld_temb=%lld must be multiples of 8", ldr, ld_temb);
   int bw, bh, bb;
   pick_box(B, H, W, &bw, &bh, &bb);
   const int m_tiles_est = (W / bw) * cdiv(H, bh) * cdiv(B, bb);

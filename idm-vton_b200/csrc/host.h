@@ -44,6 +44,10 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
+// Pointers the kernels access with 16-byte vector loads / stores (epilogue operands, norm rows) must be 16-byte aligned;
+// a null pointer (operand absent) passes.
+inline bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 // Streaming multiprocessors of the current device (read once per device: 132 on an H100 SXM, fewer on other parts).
 int num_sms();
 

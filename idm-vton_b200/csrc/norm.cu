@@ -27,9 +27,14 @@ __device__ __forceinline__ uint4 gn_load(const GnSrc& s, long long row, int v) {
   if (c < s.C0) return *reinterpret_cast<const uint4*>(s.x0 + row * s.C0 + c);
   return *reinterpret_cast<const uint4*>(s.x1 + row * s.C1 + (c - s.C0));
 }
+__device__ __forceinline__ float gn_scalar(const GnSrc& s, long long row, int c) {
+  return h2f(c < s.C0 ? s.x0[row * s.C0 + c] : s.x1[row * s.C1 + (c - s.C0)]);
+}
 
 // ONE launch per GroupNorm (round 2; round 1 ran a statistics kernel and an apply kernel = 3 passes over the tensor):
-//   phase 1: CTA (chunk, b) streams its rows once, accumulates per-channel sums / sums of squares in a fixed order and —
+//   phase 1: CTA (chunk, b) streams its rows once, accumulates per-channel sums / sums of squares of x - s_g in a fixed
+//            order (s_g = the sample's first pixel in the group's first channel, the same value for every CTA: without the
+//            shift, E[x^2] - mean^2 of fp32 sums loses the variance of a group whose mean is large against its spread) and —
 //            when its rows fit shared memory (RESIDENT) — parks the raw fp16 rows there; it publishes
 //            partial[b][chunk][g] = {sum, sum of squares} (double).
 //   barrier: the CTAs of ONE sample meet at a sense-reversing barrier in global memory (count + sense per sample; the
@@ -61,25 +66,30 @@ gn_fused_kernel(GnSrc src, int HW, int rows_per_cta, double* partial, GnBarrier*
   const int r_end = min(HW, r_begin + rows_per_cta);
   __shared__ float ps[GN_THREADS * 8];  // [row_lane][C] partial sums
   __shared__ float pq[GN_THREADS * 8];  // [row_lane][C] partial sums of squares
-  __shared__ float s_mean[GN_GROUPS], s_rstd[GN_GROUPS];
+  __shared__ float s_mean[GN_GROUPS], s_rstd[GN_GROUPS], s_shift[GN_GROUPS];
   __shared__ int s_sense;
   const int v = threadIdx.x % V;
   const int rl = threadIdx.x / V;
   if (threadIdx.x == 0) s_sense = *reinterpret_cast<volatile int*>(&bar[b].sense);   // read BEFORE anyone can flip it
-  // ---------------- phase 1: statistics (and parking the rows)
+  if (threadIdx.x < GN_GROUPS) s_shift[threadIdx.x] = gn_scalar(src, static_cast<long long>(b) * HW, threadIdx.x * cpg);
+  // ---------------- phase 1: statistics of x - s_g (and parking the rows)
   if (rl < row_lanes) {
-    float sum[8], sq[8];
+    float sum[8], sq[8], sft[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) sum[j] = sq[j] = 0.f;
+    for (int j = 0; j < 8; ++j) {
+      sum[j] = sq[j] = 0.f;
+      sft[j] = gn_scalar(src, static_cast<long long>(b) * HW, (v * 8 + j) / cpg * cpg);
+    }
     auto acc = [&](const uint4 u) {
       const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 f = unpack_h2(w[j]);
-        sum[2 * j] += f.x;
-        sq[2 * j] += f.x * f.x;
-        sum[2 * j + 1] += f.y;
-        sq[2 * j + 1] += f.y * f.y;
+        const float d0 = f.x - sft[2 * j], d1 = f.y - sft[2 * j + 1];
+        sum[2 * j] += d0;
+        sq[2 * j] += d0 * d0;
+        sum[2 * j + 1] += d1;
+        sq[2 * j + 1] += d1 * d1;
       }
     };
     int r = r_begin + rl;
@@ -198,24 +208,25 @@ gn_fused_kernel(GnSrc src, int HW, int rows_per_cta, double* partial, GnBarrier*
         tq += red_q[s2 * GN_GROUPS + threadIdx.x];
       }
       const double n = static_cast<double>(cpg) * HW;
-      const double mean = ta / n;
-      double var = tq / n - mean * mean;
+      const double dmean = ta / n;                 // mean of x - s_g
+      double var = tq / n - dmean * dmean;
       var = var < 0.0 ? 0.0 : var;
-      s_mean[threadIdx.x] = static_cast<float>(mean);
+      s_mean[threadIdx.x] = static_cast<float>(s_shift[threadIdx.x] + dmean);
       s_rstd[threadIdx.x] = rsqrtf(static_cast<float>(var) + eps);
     }
     __syncthreads();
   }
   if (rl >= row_lanes) return;
-  float sc[8], sh[8];
+  // y = x * (rstd * gamma) + (beta - mean * rstd * gamma)
+  float sc[8], sh[8], mu[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = v * 8 + j;
     const int g = c / cpg;
     const float gm = gamma ? h2f(gamma[c]) : 1.f;
-    const float bt = beta ? h2f(beta[c]) : 0.f;
     sc[j] = s_rstd[g] * gm;
-    sh[j] = bt - s_mean[g] * sc[j];
+    sh[j] = beta ? h2f(beta[c]) : 0.f;
+    mu[j] = s_mean[g];
   }
   auto apply_row = [&](int r, const uint4 u) {
     const long long row = static_cast<long long>(b) * HW + r;
@@ -224,8 +235,8 @@ gn_fused_kernel(GnSrc src, int HW, int rows_per_cta, double* partial, GnBarrier*
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = unpack_h2(w[j]);
-      y[2 * j] = f.x * sc[2 * j] + sh[2 * j];
-      y[2 * j + 1] = f.y * sc[2 * j + 1] + sh[2 * j + 1];
+      y[2 * j] = f.x * sc[2 * j] + (sh[2 * j] - mu[2 * j] * sc[2 * j]);
+      y[2 * j + 1] = f.y * sc[2 * j + 1] + (sh[2 * j + 1] - mu[2 * j + 1] * sc[2 * j + 1]);
     }
     if (silu) {
 #pragma unroll
@@ -265,6 +276,8 @@ int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW
   VTON_CHECK_ARG(C / 8 <= GN_THREADS, "groupnorm: C=%d too wide", C);
   VTON_CHECK_ARG(stats_ws != nullptr, "groupnorm: stats workspace required (see include/b200vton.h)");
   VTON_CHECK_ARG(B <= GN_MAX_BATCH_BARRIER, "groupnorm: batch %d > %d", B, GN_MAX_BATCH_BARRIER);
+  VTON_CHECK_ARG(aligned_to(x0, 16) && aligned_to(x1, 16) && aligned_to(out, 16),
+                 "groupnorm: x0/x1/out must be 16-byte aligned (rows are read and written 8 halves at a time)");
   GnSrc src{static_cast<const __half*>(x0), static_cast<const __half*>(x1), C0, C1};
   static int max_smem = 0, occ_stream = 0;
   if (!max_smem) {
@@ -396,6 +409,8 @@ int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* ga
                    void* out, long long ldo, cudaStream_t stream) {
   VTON_CHECK_ARG(rows > 0 && C > 0, "layernorm: empty input");
   VTON_CHECK_ARG(C % 8 == 0 && C <= LN_MAX_VEC * 256 && ldx % 8 == 0 && ldo % 8 == 0, "layernorm: C=%d unsupported", C);
+  VTON_CHECK_ARG(aligned_to(x, 16) && aligned_to(out, 16) && aligned_to(gamma, 16) && aligned_to(beta, 16),
+                 "layernorm: x/out/gamma/beta must be 16-byte aligned (read and written 8 halves at a time)");
   const int nv = cdiv(C / 8, 32);
   auto go = [&](auto kern) {
     return launch_kernel(kern, dim3(cdiv(rows, 8)), dim3(256), 0, stream, static_cast<const __half*>(x), ldx, rows, C,

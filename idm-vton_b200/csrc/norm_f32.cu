@@ -25,14 +25,21 @@ gn32_stats_kernel(const float* __restrict__ x, int HW, int C, int rows_per_cta, 
   const int v = threadIdx.x % V;
   const int rl = threadIdx.x / V;
   if (rl < row_lanes) {
-    float sum[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
-    const float* base = x + (static_cast<long long>(b) * HW) * C + v * 4;
+    // sums of x - s_g, s_g = the sample's first pixel in the group's first channel (the same for every CTA; see
+    // gn_fused_kernel): E[x^2] - mean^2 of unshifted fp32 sums loses the variance of a group with a large mean
+    float sum[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f}, sft[4];
+    const float* sample = x + (static_cast<long long>(b) * HW) * C;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) sft[j] = __ldg(sample + (v * 4 + j) / cpg * cpg);
+    const float* base = sample + v * 4;
     for (long long r = r_begin + rl; r < r_end; r += row_lanes) {
       const float4 u = __ldg(reinterpret_cast<const float4*>(base + r * C));
-      sum[0] += u.x; sq[0] += u.x * u.x;
-      sum[1] += u.y; sq[1] += u.y * u.y;
-      sum[2] += u.z; sq[2] += u.z * u.z;
-      sum[3] += u.w; sq[3] += u.w * u.w;
+      const float d[4] = {u.x - sft[0], u.y - sft[1], u.z - sft[2], u.w - sft[3]};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        sum[j] += d[j];
+        sq[j] += d[j] * d[j];
+      }
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -101,28 +108,31 @@ gn32_apply_kernel(const float* __restrict__ x, int HW, int C, int rows_per_cta, 
       q += red_q[sl][threadIdx.x];
     }
     const double n = static_cast<double>(cpg) * HW;
-    const double mean = a / n;
-    double var = q / n - mean * mean;
+    const double dmean = a / n;                   // mean of x - s_g
+    double var = q / n - dmean * dmean;
     var = var < 0.0 ? 0.0 : var;
-    s_mean[threadIdx.x] = static_cast<float>(mean);
+    const float shift = __ldg(x + (static_cast<long long>(b) * HW) * C + threadIdx.x * cpg);
+    s_mean[threadIdx.x] = static_cast<float>(shift + dmean);
     s_rstd[threadIdx.x] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
   }
   __syncthreads();
   if (rl >= row_lanes) return;
-  float sc[4], sh[4];
+  // y = (x - mean) * (rstd * gamma) + beta: subtracting first keeps a large mean from cancelling in fp32
+  float sc[4], sh[4], mu[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int c = v * 4 + j;
     const int g = c / cpg;
     const float gm = gamma ? gamma[c] : 1.f;
-    const float bt = beta ? beta[c] : 0.f;
     sc[j] = s_rstd[g] * gm;
-    sh[j] = bt - s_mean[g] * sc[j];
+    sh[j] = beta ? beta[c] : 0.f;
+    mu[j] = s_mean[g];
   }
   const long long off = (static_cast<long long>(b) * HW) * C + v * 4;
   for (long long r = r_begin + rl; r < r_end; r += row_lanes) {
     const float4 u = __ldg(reinterpret_cast<const float4*>(x + off + r * C));
-    float y[4] = {u.x * sc[0] + sh[0], u.y * sc[1] + sh[1], u.z * sc[2] + sh[2], u.w * sc[3] + sh[3]};
+    float y[4] = {fmaf(u.x - mu[0], sc[0], sh[0]), fmaf(u.y - mu[1], sc[1], sh[1]), fmaf(u.z - mu[2], sc[2], sh[2]),
+                  fmaf(u.w - mu[3], sc[3], sh[3])};
     if (silu) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) y[j] = silu_f(y[j]);
@@ -138,7 +148,8 @@ gn32_apply_kernel(const float* __restrict__ x, int HW, int C, int rows_per_cta, 
   }
 }
 
-// x: [B, HW, C] fp32 dense NHWC; out: the same shape, fp32 or (out_fp16) fp16; gamma/beta: [C] fp32 or null;
+// x: [B, HW, C] fp32 dense NHWC; out: the same shape, fp32 or (out_fp16) fp16, and must not alias x (every apply CTA
+// re-reads the shift in row 0 of its sample, which CTA 0 overwrites); gamma/beta: [C] fp32 or null;
 // stats_ws: B * chunks(<= 1184) * 64 doubles
 int groupnorm_f32_impl(const void* x, int B, int HW, int C, const void* gamma, const void* beta, float eps, int silu,
                        void* stats_ws, long long stats_ws_doubles, void* out, int out_fp16, cudaStream_t stream) {

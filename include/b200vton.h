@@ -120,7 +120,7 @@ int b200vton_softmax_split_tf32(const void* scores, int64_t rows, int N, void* p
  * ResnetBlock2D.norm1/norm2 + SiLU, Attention.group_norm, conv_norm_out), deterministic two-stage statistics.
  * gamma/beta: [C] fp32 or NULL. stats_ws: scratch of stats_ws_doubles doubles, at least 64 * max(B, 1184) is always
  * enough. out: fp32, or — out_fp16 != 0 — fp16 of the same shape (one rounding of the fp32 result), the operand format of
- * b200vton_conv3x3_nhwc_f16in_f32. The VAE's default route (B200VTON_VAE_NHWC=0 restores the cuDNN NCHW path). */
+ * b200vton_conv3x3_nhwc_f16in_f32; out must not alias x (no in-place call). The VAE's default route (B200VTON_VAE_NHWC=0 restores the cuDNN NCHW path). */
 int b200vton_groupnorm_nhwc_f32(const void* x, int B, int HW, int C, const void* gamma, const void* beta, float eps,
                                  int silu, void* stats_ws, int64_t stats_ws_doubles, void* out, int out_fp16, void* stream);
 

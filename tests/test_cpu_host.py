@@ -628,6 +628,46 @@ def test_library_options_and_argument_checks_without_gpu():
     assert rc == 1 and b"multiples of 32" in l.b200vton_last_error()
     assert l.b200vton_split_tf32(None, 6, 1, 6, 1.0, None, None, None) == 1 and b"split_tf32" in l.b200vton_last_error()
     assert l.b200vton_softmax_split_tf32(None, 4, 6, None, None, None) == 1
+    # operands the kernels access with 16-byte vectors (4-byte stores for attention's out) must be aligned, and the row
+    # strides of residual / rowvec / temb multiples of 8 halves: refused before any tensor map is encoded or anything
+    # launched (fake device addresses, never dereferenced)
+    A, OK, BAD, BAD4 = 0x10000, 0x20000, 0x20008, 0x20002
+    gemm = l.b200vton_gemm_f16
+    for kw in ("out", "bias", "residual", "rowvec"):
+        ptr = {k: OK for k in ("out", "bias", "residual", "rowvec")}
+        ptr[kw] = BAD
+        rc = gemm(A, 64, A, 64, ptr["out"], 64, 128, 64, 64, ptr["bias"], ptr["residual"], 64, ptr["rowvec"], 64, 128, 0,
+                  0, None)
+        assert rc == 1 and b"16-byte aligned" in l.b200vton_last_error(), kw
+    assert gemm(A, 64, A, 64, OK, 64, 128, 64, 64, None, OK, 68, None, 0, 0, 0, 0, None) == 1
+    assert b"ldr=68" in l.b200vton_last_error()
+    assert gemm(A, 64, A, 64, OK, 64, 128, 64, 64, None, None, 0, OK, 36, 77, 0, 0, None) == 1
+    assert b"ld_rowvec=36" in l.b200vton_last_error()
+    conv = l.b200vton_conv3x3_nhwc
+    for kw in ("out", "bias", "temb", "bias_sc", "residual"):
+        ptr = {k: OK for k in ("out", "bias", "temb", "bias_sc", "residual")}
+        ptr[kw] = BAD
+        sc = kw == "bias_sc"          # a shortcut and an identity residual are exclusive
+        rc = conv(A, 64, 1, 8, 8, 64, A, 64, ptr["bias"], ptr["temb"], 64, A if sc else None, 64 if sc else 0, None, 0,
+                  A if sc else None, ptr["bias_sc"] if sc else None, None if sc else ptr["residual"], 64, ptr["out"], 64,
+                  0, 1, None)
+        assert rc == 1 and b"16-byte aligned" in l.b200vton_last_error(), kw
+    assert conv(A, 64, 2, 8, 8, 64, A, 64, None, OK, 1284, None, 0, None, 0, None, None, None, 0, OK, 64, 0, 1, None) == 1
+    assert b"ld_temb=1284" in l.b200vton_last_error()
+    assert conv(A, 64, 1, 8, 8, 64, A, 64, None, None, 0, None, 0, None, 0, None, None, OK, 60, OK, 64, 0, 1, None) == 1
+    assert b"ldr=60" in l.b200vton_last_error()
+    rc = l.b200vton_attention(A, 64, A, A, 64, None, None, 0, BAD4, 64, 1, 1, 128, 128, 0, 0, 0, 0, None, 0.125, 0, None)
+    assert rc == 1 and b"4-byte aligned" in l.b200vton_last_error()
+    rc = l.b200vton_cross_attention(A, 64, A, A, 64, 77, None, None, 0, 0, BAD4, 64, 1, 1, 128, 0.125, 1.0, None)
+    assert rc == 1 and b"4-byte aligned" in l.b200vton_last_error()
+    rc = l.b200vton_encoder_attention(A, 64, A, A, 64, BAD4, 64, 1, 1, 77, 64, 0.125, 1, None)
+    assert rc == 1 and b"4-byte aligned" in l.b200vton_last_error()
+    for x0, x1, out in ((BAD, None, OK), (OK, BAD, OK), (OK, OK, BAD)):
+        rc = l.b200vton_groupnorm(x0, 320, x1, 64 if x1 else 0, 1, 64, None, None, 1e-5, 1, OK, out, None)
+        assert rc == 1 and b"16-byte aligned" in l.b200vton_last_error()
+    for x, g, b, out in ((BAD, None, None, OK), (OK, BAD, None, OK), (OK, None, BAD, OK), (OK, None, None, BAD)):
+        rc = l.b200vton_layernorm(x, 640, 4, 640, g, b, 1e-5, out, 640, None)
+        assert rc == 1 and b"16-byte aligned" in l.b200vton_last_error()
 
 
 def test_vae_conv_dispatch_and_weight_packing_on_cpu():
