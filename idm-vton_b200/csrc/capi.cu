@@ -52,13 +52,15 @@ void set_attn_qtiles(int n);
 void set_attn_poly(int n);
 int cfg_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
                   const void* coef, int do_cfg, void* out, cudaStream_t stream);
+int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                          const void* coef, int do_cfg, void* out, cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
 
 extern "C" {
 
-int b200vton_version(void) { return 106; }
+int b200vton_version(void) { return 107; }
 const char* b200vton_last_error(void) { return vton::get_last_error(); }
 long long b200vton_launch_count(void) { return vton::launch_count(); }
 int b200vton_set_option(const char* name, int value) {
@@ -188,6 +190,10 @@ int b200vton_skinny_linear(const void* x, int ldx, int M, int K, const void* W, 
 int b200vton_cfg_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
                            const void* noise, const void* coef, int do_cfg, void* out, void* stream) {
   return vton::cfg_ddpm_impl(eps, ldc, B, C, H, W, latents, noise, coef, do_cfg, out, S(stream));
+}
+int b200vton_cfg_rescale_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                   const void* noise, const void* coef, int do_cfg, void* out, void* stream) {
+  return vton::cfg_rescale_ddpm_impl(eps, ldc, B, C, H, W, latents, noise, coef, do_cfg, out, S(stream));
 }
 
 int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_channels, const void* image_min, int B,

@@ -270,6 +270,103 @@ int cfg_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const vo
 }
 
 // ------------------------------------------------------------------------------------------------
+// CFG + guidance rescale + DDPM step (src/tryon_pipeline.py:101-113 rescale_noise_cfg, applied at :1818-1820; the
+// "Common Diffusion Noise Schedules and Sample Steps are Flawed" correction). One CTA per sample b:
+//   g   = u + fp16(gs * fp16(t - u))                                  (the CFG result of cfg_ddpm_kernel)
+//   s_t = fp16(std(t)), s_g = fp16(std(g))   unbiased (torch.std's default), over the C*H*W values of sample b
+//   r   = fp16(s_t / s_g)
+//   g'  = fp16(fp16(phi * fp16(g * r)) + fp16((1 - phi) * g))
+// then cfg_ddpm_kernel's DDPM update on g'. These are the rounding points of the reference's fp16 tensor arithmetic on the
+// fp16 noise_pred inside torch.autocast(float16): std of an fp16 tensor returns fp16 there (statistics accumulated in
+// fp32 by torch, the result rounded). The statistics here are two-pass (mean, then squared deviations) in double, each
+// thread over a fixed strided subset and a fixed-shape tree across the CTA: the result does not depend on timing, and
+// there are no atomics. coef: 7 floats {gs, sb, inv_sa, c0, c1, sigma, phi} on the device (graph-replayable).
+// ------------------------------------------------------------------------------------------------
+constexpr int kRescaleThreads = 1024;
+
+// Sum of v over the CTA in a fixed order; every thread gets the result. red: kRescaleThreads / 32 doubles of shared.
+__device__ __forceinline__ double cta_sum(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();                     // red may still be read by the previous call
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = lane < (kRescaleThreads >> 5) ? red[lane] : 0.0;
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_ddpm_kernel(
+    const __half* eps, int ldc, int B, int C, int HW, const __half* latents, const __half* noise, const float* coef,
+    __half* out) {
+  __shared__ double red[kRescaleThreads / 32];
+  const int b = blockIdx.x;
+  const float gs = coef[0], sb = coef[1], inv_sa = coef[2], c0 = coef[3], c1 = coef[4], sigma = coef[5], phi = coef[6];
+  const __half* eu = eps + static_cast<long long>(b) * HW * ldc;         // uncond rows of sample b
+  const __half* et = eps + static_cast<long long>(b + B) * HW * ldc;     // cond rows of sample b
+  const int n = C * HW;
+  // the CFG result, from the same fp16 values the apply pass reads
+  auto cfg = [&](long long off, float& t) {
+    const float u = h2f(eu[off]);
+    t = h2f(et[off]);
+    return round_h(u + round_h(gs * round_h(t - u)));
+  };
+  // pass 1: means (NHWC order: consecutive threads read consecutive channels / pixels)
+  double st = 0.0, sg = 0.0;
+  for (int k = threadIdx.x; k < n; k += kRescaleThreads) {
+    const long long off = static_cast<long long>(k / C) * ldc + k % C;
+    float t;
+    const float g = cfg(off, t);
+    st += t;
+    sg += g;
+  }
+  const double mt = cta_sum(st, red) / n;
+  const double mg = cta_sum(sg, red) / n;
+  // pass 2: sums of squared deviations
+  double qt = 0.0, qg = 0.0;
+  for (int k = threadIdx.x; k < n; k += kRescaleThreads) {
+    const long long off = static_cast<long long>(k / C) * ldc + k % C;
+    float t;
+    const float g = cfg(off, t);
+    qt += (t - mt) * (t - mt);
+    qg += (g - mg) * (g - mg);
+  }
+  qt = cta_sum(qt, red);
+  qg = cta_sum(qg, red);
+  // n == 1 gives 0/0 = NaN like torch.std of one value
+  const float s_t = round_h(static_cast<float>(sqrt(qt / (n - 1))));
+  const float s_g = round_h(static_cast<float>(sqrt(qg / (n - 1))));
+  const float r = round_h(s_t / s_g);
+  // pass 3: rescale + DDPM update, NCHW order over the latents / noise / out
+  const long long base = static_cast<long long>(b) * n;
+  for (int k = threadIdx.x; k < n; k += kRescaleThreads) {
+    const int c = k / HW, px = k % HW;
+    float t;
+    const float g = cfg(static_cast<long long>(px) * ldc + c, t);
+    const float gr = round_h(round_h(phi * round_h(g * r)) + round_h((1.0f - phi) * g));
+    const float x = h2f(latents[base + k]);
+    const float x0 = round_h(round_h(x - round_h(sb * gr)) * inv_sa);
+    float prev = round_h(round_h(c0 * x0) + round_h(c1 * x));
+    if (noise) prev = round_h(prev + round_h(sigma * h2f(noise[base + k])));
+    out[base + k] = f2h(prev);
+  }
+}
+
+int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                          const void* coef, int do_cfg, void* out, cudaStream_t stream) {
+  // without CFG there is no rescale (the reference applies it only under CFG): the plain step, phi unused
+  if (!do_cfg) return cfg_ddpm_impl(eps, ldc, B, C, H, W, latents, noise, coef, 0, out, stream);
+  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef, "cfg_rescale_ddpm: bad arguments");
+  VTON_CHECK_ARG(static_cast<long long>(C) * H * W < (1LL << 31), "cfg_rescale_ddpm: sample too large");
+  cfg_rescale_ddpm_kernel<<<B, kRescaleThreads, 0, stream>>>(
+      static_cast<const __half*>(eps), ldc, B, C, H * W, static_cast<const __half*>(latents),
+      static_cast<const __half*>(noise), static_cast<const float*>(coef), static_cast<__half*>(out));
+  count_launch();
+  VTON_CUDA(cudaGetLastError());
+  return kOk;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Pre / post-processing around the VAE (SURVEY.md 8f item 3; diffusers VaeImageProcessor as the pipeline uses it,
 // src/tryon_pipeline.py:418-421, 1588-1602, 940-955, 1885). One launch each instead of ~10 small ATen kernels.
 //   preprocess: image [B,3,H,W] fp32 -> init_image = 2x-1 (skipped when the batch already has negative values: diffusers

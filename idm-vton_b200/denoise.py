@@ -3,7 +3,7 @@
 Per step the reference runs the garment UNet (batch Bg), zero-pads its 70 features for the CFG-uncond half, runs the
 try-on UNet (batch 2B), applies CFG and the DDPM update. Here one step is a fixed launch sequence over static buffers:
   latents -> [NCHW->NHWC scatter into the 13(+pad)-channel input] -> garment UNet -> try-on UNet (garment K/V streamed
-  as a second attention segment, uncond half in closed form) -> fused CFG+DDPM
+  as a second attention segment, uncond half in closed form) -> fused CFG(+guidance rescale)+DDPM
 captured once in a CUDA graph and replayed per step; step-invariant work (cross-attention K/V of text / IP tokens,
 aug_emb, the static input channels) is hoisted to prepare().
 """
@@ -30,7 +30,9 @@ def ddpm_step_coefficients(scheduler, t):
     fp32 torch like diffusers does, from the GENERIC scheduler interface only — `alphas_cumprod`,
     `config.num_train_timesteps`, `num_inference_steps` (and `previous_timestep` when the object has it) — so the
     caller's own `diffusers.DDPMScheduler` works (inference.py passes `DDPMScheduler.from_pretrained(...)`). The fused
-    kernel implements epsilon prediction with fixed_small variance and no clipping / thresholding: anything else raises."""
+    kernel implements epsilon prediction with fixed_small variance and no clipping / thresholding: anything else raises.
+    A custom timestep list (`custom_timesteps`) needs `previous_timestep`: the even spacing t - T_train // steps would
+    be wrong for it."""
     cfg = getattr(scheduler, "config", None)
     get = (lambda k, d=None: cfg.get(k, d)) if isinstance(cfg, dict) else (lambda k, d=None: getattr(cfg, k, d))
     if get("prediction_type", "epsilon") != "epsilon" or get("variance_type", "fixed_small") != "fixed_small" \
@@ -43,6 +45,9 @@ def ddpm_step_coefficients(scheduler, t):
     n_train = int(get("num_train_timesteps", len(scheduler.alphas_cumprod)))
     if hasattr(scheduler, "previous_timestep"):
         prev_t = int(scheduler.previous_timestep(t))
+    elif getattr(scheduler, "custom_timesteps", False):
+        raise TypeError(f"{type(scheduler).__name__} has a custom timestep list but no previous_timestep(): the step "
+                        "from each timestep to the next cannot be derived")
     else:
         steps = getattr(scheduler, "num_inference_steps", None) or n_train
         prev_t = t - n_train // steps
@@ -121,33 +126,39 @@ class TryOnDenoiser:
 
     # -------------------------------------------------------------------------------------------
     def prepare(self, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds,
-                add_text_embeds, add_time_ids, image_embeds, text_embeds_cloth, guidance_scale=2.0, do_cfg=True):
-        """All tensors on the device. latents [B,4,h,w]; mask [Bt,1,h,w], masked_image_latents / pose_latents
+                add_text_embeds, add_time_ids, image_embeds, text_embeds_cloth, guidance_scale=2.0, do_cfg=True,
+                guidance_rescale=0.0):
+        """guidance_rescale: phi of rescale_noise_cfg (src/tryon_pipeline.py:101-113), applied only under CFG; 0 keeps
+        the plain CFG+DDPM kernel. All tensors on the device. latents [B,4,h,w]; mask [Bt,1,h,w], masked_image_latents / pose_latents
         [Bt,4,h,w], prompt_embeds [Bt,77,X], add_text_embeds [Bt,P], add_time_ids [Bt,6], image_embeds [Bt,16,X]
         with Bt = 2B under CFG ([uncond ; cond] order, src/tryon_pipeline.py:1711-1714); cloth_latents [Bg,4,h,w],
         text_embeds_cloth [Bg,77,X]."""
         torch.cuda.nvtx.range_push("b200vton.prepare(context K/V, aug_emb, static input channels)")
         try:
             self._prepare(latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
-                          add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg)
+                          add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg, guidance_rescale)
         finally:
             torch.cuda.nvtx.range_pop()
 
     def _prepare(self, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
-                 add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg):
+                 add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg, guidance_rescale):
         L = self.L
         f16 = torch.float16
         B, _, h, w = latents.shape
         Bt = 2 * B if do_cfg else B
         Bg = cloth_latents.shape[0]
         dev = self.device
-        key = (B, Bt, Bg, h, w, bool(do_cfg), tuple(prompt_embeds.shape), tuple(image_embeds.shape),
+        # the rescale flag selects the step's last kernel: a graph captured with the other one must not be replayed
+        rescale = bool(do_cfg) and guidance_rescale > 0
+        key = (B, Bt, Bg, h, w, bool(do_cfg), rescale, tuple(prompt_embeds.shape), tuple(image_embeds.shape),
                tuple(text_embeds_cloth.shape))
         fresh = key != getattr(self, "_key", None)
         self._key = key
         self.B, self.Bt, self.Bg, self.h, self.w = B, Bt, Bg, h, w
         self.do_cfg = do_cfg
         self.guidance_scale = float(guidance_scale)
+        self.rescale = rescale
+        self.guidance_rescale = float(guidance_rescale)
         if fresh:
             # (re)allocate every static buffer the step graph points at; same-shaped requests reuse them (and the
             # captured graph) and only overwrite their contents
@@ -159,7 +170,7 @@ class TryOnDenoiser:
             self.x_t = torch.zeros((Bt, h, w, CIN_PAD), dtype=f16, device=dev)
             self.x_g = torch.zeros((Bg, h, w, CIN_PAD), dtype=f16, device=dev)
             self.t_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-            self.coef = torch.zeros(6, dtype=torch.float32, device=dev)
+            self.coef = torch.zeros(7, dtype=torch.float32, device=dev)
             self.step_base = torch.zeros(1, dtype=torch.int32, device=dev)   # step index * Bg (hoisted garment K/V)
             self.ctx_t = self.ctx_g = self.aug = None
             self.eps = None
@@ -173,13 +184,13 @@ class TryOnDenoiser:
         self.aug = self.tryon.aug_embedding(add_text_embeds.to(dev, f16), add_time_ids.to(dev), out=self.aug)
 
     def set_step_tables(self, scheduler, timesteps, garment_keys=None, cache=None):
-        """Uploads the per-step scalars: t and {gs, sqrt(1-abar), 1/sqrt(abar), c0, c1, sigma}, then runs the hoisted
+        """Uploads the per-step scalars: t and {gs, sqrt(1-abar), 1/sqrt(abar), c0, c1, sigma, phi}, then runs the hoisted
         garment passes. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments whose
         K/V of all steps are cached are copied in instead of recomputed — valid only when the caller guarantees that a
         key identifies (cloth latents, text_embeds_cloth); the timestep list and latent size are added to the key here."""
         rows = []
         for t in timesteps:
-            rows.append([self.guidance_scale, *ddpm_step_coefficients(scheduler, int(t))])
+            rows.append([self.guidance_scale, *ddpm_step_coefficients(scheduler, int(t)), self.guidance_rescale])
         self.coef_table = torch.tensor(rows, dtype=torch.float32, device=self.device)
         self.t_table = torch.tensor([float(int(t)) for t in timesteps], dtype=torch.float32, device=self.device)
         T = len(rows)
@@ -287,7 +298,8 @@ class TryOnDenoiser:
             temb_g = self.garment.time_embedding(self.t_dev, self.Bg)
             self.garment.forward(self.x_g, temb_g, self.ctx_g, collect=feats)
             self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=n_persons)
-        L.cfg_ddpm_step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
+        step = L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
+        step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
         self.latents.copy_(self.latents_next)
 
     # Programmatic dependent launch INSIDE the captured step only (B200VTON_PDL_GRAPH, default below): every kernel node

@@ -39,12 +39,13 @@ SIGNATURES = {
     "b200vton_timestep_embedding": [_vp, _i, _i, _i, _vp, _vp],
     "b200vton_skinny_linear": [_vp, _i, _i, _i, _vp, _i64, _i, _vp, _i, _i, _vp, _i, _vp, _i, _vp],
     "b200vton_cfg_ddpm_step": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp],
+    "b200vton_cfg_rescale_ddpm_step": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp],
     "b200vton_preprocess_inpaint": [_vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "b200vton_postprocess_image": [_vp, _i, _i, _i, _i, _vp, _vp, _vp],
 }
 
 _lib = None
-ABI_VERSION = 106      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
+ABI_VERSION = 107      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
 
 
 def load(build_if_missing=True):
@@ -492,6 +493,18 @@ def cfg_ddpm_step(eps, latents, noise, coef, do_cfg=True, out=None):
     rc = lib.b200vton_cfg_ddpm_step(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(coef), int(do_cfg),
                                     _p(out), _stream())
     _check(rc, "b200vton_cfg_ddpm_step")
+    return out
+
+
+def cfg_rescale_ddpm_step(eps, latents, noise, coef, do_cfg=True, out=None):
+    """cfg_ddpm_step with guidance rescale; coef: 7 fp32 on device (the 6 of cfg_ddpm_step, then guidance_rescale)."""
+    lib = load()
+    B, C, H, W = latents.shape
+    if out is None:
+        out = torch.empty_like(latents)
+    rc = lib.b200vton_cfg_rescale_ddpm_step(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(coef),
+                                            int(do_cfg), _p(out), _stream())
+    _check(rc, "b200vton_cfg_rescale_ddpm_step")
     return out
 
 

@@ -420,7 +420,10 @@ class StableDiffusionXLInpaintPipeline:
     def prepare_latents(self, batch_size, num_channels_latents, height, width, dtype, device, generator, latents=None,
                         image=None, timestep=None, is_strength_max=True, add_noise=True, return_noise=False,
                         return_image_latents=False):
-        """src/tryon_pipeline.py:850-909 (strength < 1 needs scheduler.add_noise: not on the inference.py path)."""
+        """src/tryon_pipeline.py:850-909. strength < 1: the image is encoded (user generator) before the noise is drawn,
+        and the latents are the image latents noised to `timestep` by `scheduler.add_noise`; add_noise=False
+        (denoising_start): the noise is still drawn and the latents are the image latents; latents given by the caller
+        are noise, scaled by init_noise_sigma."""
         shape = (batch_size, num_channels_latents, height // self.vae_scale_factor, width // self.vae_scale_factor)
         if isinstance(generator, list) and len(generator) != batch_size:
             raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an effective batch"
@@ -428,20 +431,28 @@ class StableDiffusionXLInpaintPipeline:
         if (image is None or timestep is None) and not is_strength_max:
             raise ValueError("Since strength < 1. initial latents are to be initialised as a combination of Image + Noise."
                              "However, either the image or the noise timestep has not been provided.")
-        if not is_strength_max or not add_noise:
-            raise NotImplementedError("strength < 1 / denoising_start are not on the IDM-VTON inference path")
         image_latents = None
         if image.shape[1] == 4:
             image_latents = image.to(device=device, dtype=dtype).repeat(batch_size // image.shape[0], 1, 1, 1)
-        elif return_image_latents:
+        elif return_image_latents or (latents is None and not is_strength_max):
             image_latents = self._encode_vae_image(image.to(device=device, dtype=dtype), generator)
             image_latents = image_latents.repeat(batch_size // image_latents.shape[0], 1, 1, 1)
-        if latents is None:
+        if latents is None and add_noise:
             noise = randn_tensor(shape, generator=generator, device=device, dtype=dtype)
-            latents = noise * self.scheduler.init_noise_sigma
-        else:
+            if is_strength_max:
+                latents = noise * self.scheduler.init_noise_sigma
+            else:
+                latents = self.scheduler.add_noise(image_latents, noise, timestep)
+        elif add_noise:
             noise = latents.to(device)
             latents = noise * self.scheduler.init_noise_sigma
+        else:
+            if image_latents is None:
+                # the reference fails here with an unbound variable: denoising_start needs the image encoded, which
+                # happens only for strength < 1 without caller latents
+                raise ValueError("denoising_start starts from the image latents: it needs strength < 1 and no `latents`")
+            noise = randn_tensor(shape, generator=generator, device=device, dtype=dtype)
+            latents = image_latents.to(device)
         outputs = (latents,)
         if return_noise:
             outputs += (noise,)
@@ -481,13 +492,42 @@ class StableDiffusionXLInpaintPipeline:
         return mask, masked_image_latents
 
     def get_timesteps(self, num_inference_steps, strength, device, denoising_start=None):
-        """src/tryon_pipeline.py:983-1016 (denoising_start unsupported here)."""
-        if denoising_start is not None:
-            raise NotImplementedError("denoising_start is not on the IDM-VTON inference path")
-        init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
-        t_start = max(num_inference_steps - init_timestep, 0)
+        """src/tryon_pipeline.py:983-1020: strength drops the first steps; denoising_start instead keeps the timesteps
+        below round(T_train * (1 - denoising_start))."""
+        if denoising_start is None:
+            init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
+            t_start = max(num_inference_steps - init_timestep, 0)
+        else:
+            t_start = 0
         timesteps = self.scheduler.timesteps[t_start * self.scheduler.order:]
+        if denoising_start is not None:
+            n_train = self.scheduler.config.num_train_timesteps
+            discrete_timestep_cutoff = int(round(n_train - (denoising_start * n_train)))
+            num_inference_steps = (timesteps < discrete_timestep_cutoff).sum().item()
+            if self.scheduler.order == 2 and num_inference_steps % 2 == 0:
+                num_inference_steps = num_inference_steps + 1     # end after the 2nd-order step, not between its halves
+            timesteps = timesteps[-num_inference_steps:]
+            return timesteps, num_inference_steps
         return timesteps, num_inference_steps - t_start
+
+    def _denoising_value_valid(self, dnv):
+        """src/tryon_pipeline.py:1558-1559, quirk included: the type test is on denoising_end for either value."""
+        return isinstance(self.denoising_end, float) and 0 < dnv < 1
+
+    def _apply_denoising_end(self, timesteps, num_inference_steps):
+        """src/tryon_pipeline.py:1732-1752: keep the timesteps >= round(T_train * (1 - denoising_end)); a float
+        denoising_start >= denoising_end is an error."""
+        start, end = self.denoising_start, self.denoising_end
+        if (end is not None and start is not None and self._denoising_value_valid(end) and self._denoising_value_valid(start)
+                and start >= end):
+            raise ValueError(f"`denoising_start`: {start} cannot be larger than or equal to `denoising_end`: "
+                             + f" {end} when using type float.")
+        elif end is not None and self._denoising_value_valid(end):
+            n_train = self.scheduler.config.num_train_timesteps
+            discrete_timestep_cutoff = int(round(n_train - (end * n_train)))
+            num_inference_steps = len(list(filter(lambda ts: ts >= discrete_timestep_cutoff, timesteps)))
+            timesteps = timesteps[:num_inference_steps]
+        return timesteps, num_inference_steps
 
     def _get_add_time_ids(self, original_size, crops_coords_top_left, target_size, aesthetic_score,
                           negative_aesthetic_score, negative_original_size, negative_crops_coords_top_left,
@@ -574,9 +614,6 @@ class StableDiffusionXLInpaintPipeline:
         self._denoising_end = denoising_end
         self._denoising_start = denoising_start
         self._interrupt = False
-        if guidance_rescale > 0.0 or denoising_end is not None or denoising_start is not None or timesteps is not None:
-            raise NotImplementedError("guidance_rescale / denoising_start / denoising_end / custom timesteps are not on the "
-                                      "IDM-VTON inference path (inference.py:397-414)")
         if cloth is None or pose_img is None or text_embeds_cloth is None:
             raise ValueError("cloth, pose_img and text_embeds_cloth are required (src/tryon_pipeline.py:1644-1654,1787)")
 
@@ -598,9 +635,11 @@ class StableDiffusionXLInpaintPipeline:
             negative_prompt_embeds=negative_prompt_embeds, pooled_prompt_embeds=pooled_prompt_embeds,
             negative_pooled_prompt_embeds=negative_pooled_prompt_embeds, clip_skip=self.clip_skip)
 
-        # 4. timesteps
+        # 4. timesteps. Reference quirk (src/tryon_pipeline.py:1558-1566): the expression meant to drop an invalid
+        # denoising_start tests the validity function itself, which is always true, so get_timesteps gets it as given
         timesteps, num_inference_steps = retrieve_timesteps(self.scheduler, num_inference_steps, device, timesteps)
-        timesteps, num_inference_steps = self.get_timesteps(num_inference_steps, strength, device)
+        timesteps, num_inference_steps = self.get_timesteps(num_inference_steps, strength, device,
+                                                            denoising_start=self.denoising_start)
         if num_inference_steps < 1:
             raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of pipeline"
                              f"steps is {num_inference_steps} which is < 1 and not appropriate for this pipeline.")
@@ -628,15 +667,16 @@ class StableDiffusionXLInpaintPipeline:
             else:
                 masked_image = init_image * (mask.to(init_image.device) < 0.5)
 
-        # 6. latents (RNG draw #1)
+        # 6. latents (RNG draw #1; with strength < 1 the image-latents sample comes first, then the noise)
         num_channels_latents = self.vae.config.latent_channels
         num_channels_unet = self.unet.config.in_channels
         if num_channels_unet != 13:
             raise NotImplementedError("the try-on UNet has 13 input channels (src/tryon_pipeline.py:1776-1777)")
         latents, noise = self.prepare_latents(batch_size * num_images_per_prompt, num_channels_latents, height, width,
                                               prompt_embeds.dtype, device, generator, latents, image=init_image,
-                                              timestep=latent_timestep, is_strength_max=is_strength_max, add_noise=True,
-                                              return_noise=True, return_image_latents=False)
+                                              timestep=latent_timestep, is_strength_max=is_strength_max,
+                                              add_noise=self.denoising_start is None, return_noise=True,
+                                              return_image_latents=False)
         # 7. mask latents (RNG draw #2), pose latents (global RNG!), cloth latents (RNG draw #3)
         pose_img = pose_img.to(device=device, dtype=prompt_embeds.dtype)
         cloth_is_latents = cloth.shape[1] == self.vae.config.latent_channels
@@ -717,6 +757,7 @@ class StableDiffusionXLInpaintPipeline:
         if trace:
             trace.mark("clip_image_encoder+resampler")
         # 11. denoising loop on the engine
+        timesteps, num_inference_steps = self._apply_denoising_end(timesteps, num_inference_steps)
         self._num_timesteps = len(timesteps)
         # unet.engine() re-packs after load_state_dict() / .to() on the module; a denoiser built on older engines (and its
         # captured graph) would silently run stale weights
@@ -726,7 +767,7 @@ class StableDiffusionXLInpaintPipeline:
         den = self._denoiser
         den.prepare(latents, mask, masked_image_latents, pose_img, cloth, prompt_embeds, add_text_embeds, add_time_ids,
                     image_embeds, text_embeds_cloth.to(device), guidance_scale=self.guidance_scale,
-                    do_cfg=self.do_classifier_free_guidance)
+                    do_cfg=self.do_classifier_free_guidance, guidance_rescale=self.guidance_rescale)
         den.set_step_tables(self.scheduler, timesteps, garment_keys=garment_keys, cache=self.garment_cache)
         if trace:
             trace.mark("denoiser.prepare (context K/V, garment passes)")

@@ -3,7 +3,8 @@
 Restates diffusers==0.25.0 DDPMScheduler as used by src/tryon_pipeline.py:1561,1823 (set_timesteps / step) for:
 scaled_linear betas 0.00085..0.012, 1000 train steps, epsilon prediction, fixed_small variance, leading spacing with
 steps_offset 1, optional zero-terminal-SNR rescale (train_xl.py:317). The per-step arithmetic itself runs in
-b200vton_cfg_ddpm_step; this class only produces the timestep list and the per-step scalar coefficients.
+b200vton_cfg_ddpm_step; this class produces the timestep list (or takes a custom one), the per-step scalar coefficients
+and the forward-process noising of add_noise (strength < 1).
 """
 import torch
 
@@ -47,12 +48,28 @@ class DDPMScheduler:
         self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
         self.one = torch.tensor(1.0)
         self.num_inference_steps = None
+        self.custom_timesteps = False
         self.timesteps = torch.arange(num_train_timesteps - 1, -1, -1)
 
-    def set_timesteps(self, num_inference_steps, device=None):
+    def set_timesteps(self, num_inference_steps=None, device=None, timesteps=None):
+        """diffusers 0.25 semantics: either a step count (spaced by `timestep_spacing`) or a custom list of train
+        timesteps, strictly descending and below num_train_timesteps (`custom_timesteps` is then set)."""
         n = self.config.num_train_timesteps
+        if num_inference_steps is not None and timesteps is not None:
+            raise ValueError("Can only pass one of `num_inference_steps` or `custom_timesteps`.")
+        if timesteps is not None:
+            ts = [int(t) for t in timesteps]
+            if any(a <= b for a, b in zip(ts, ts[1:])):
+                raise ValueError("`custom_timesteps` must be in descending order.")
+            if ts[0] >= n:
+                raise ValueError(f"`timesteps` must start before `self.config.train_timesteps`: {n}.")
+            self.custom_timesteps = True
+            ts = torch.tensor(ts, dtype=torch.int64)
+            self.timesteps = ts.to(device) if device is not None else ts
+            return
         if num_inference_steps > n:
             raise ValueError(f"num_inference_steps {num_inference_steps} > num_train_timesteps {n}")
+        self.custom_timesteps = False
         self.num_inference_steps = num_inference_steps
         sp = self.config.timestep_spacing
         if sp == "leading":
@@ -66,10 +83,24 @@ class DDPMScheduler:
             ts = torch.linspace(0, n - 1, num_inference_steps, dtype=torch.float64).round().flip(0).to(torch.int64)
         self.timesteps = ts.to(device) if device is not None else ts
 
+    def add_noise(self, original_samples, noise, timesteps):
+        """sqrt(abar_t) * x0 + sqrt(1 - abar_t) * noise per sample, with alphas_cumprod cast to the samples' dtype and
+        device first (diffusers DDPMScheduler.add_noise)."""
+        ac = self.alphas_cumprod.to(device=original_samples.device, dtype=original_samples.dtype)
+        timesteps = timesteps.to(original_samples.device)
+        sqrt_a = ac[timesteps] ** 0.5
+        sqrt_1ma = (1 - ac[timesteps]) ** 0.5
+        shape = (-1,) + (1,) * (original_samples.ndim - 1)
+        return sqrt_a.reshape(shape) * original_samples + sqrt_1ma.reshape(shape) * noise
+
     def scale_model_input(self, sample, timestep=None):
         return sample
 
     def previous_timestep(self, t):
+        if self.custom_timesteps:
+            ts = self.timesteps.tolist()
+            i = ts.index(int(t))
+            return ts[i + 1] if i + 1 < len(ts) else -1
         steps = self.num_inference_steps if self.num_inference_steps else self.config.num_train_timesteps
         return t - self.config.num_train_timesteps // steps
 

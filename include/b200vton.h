@@ -193,6 +193,14 @@ int b200vton_token_embedding(const void* ids, int rows, int T, int C, int vocab,
 int b200vton_cfg_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
                            const void* noise, const void* coef, int do_cfg, void* out, void* stream);
 
+/* b200vton_cfg_ddpm_step with guidance rescale between the CFG combine and the DDPM step (rescale_noise_cfg,
+ * src/tryon_pipeline.py:101-113,1818-1820): per sample, g' = phi * g * std(cond)/std(g) + (1 - phi) * g with unbiased
+ * std over C*H*W, in the reference's fp16 rounding points. Same layout as b200vton_cfg_ddpm_step; coef: 7 fp32 on
+ * device {the 6 above, phi}. One CTA per sample, deterministic reductions, graph-capturable. do_cfg == 0 runs
+ * b200vton_cfg_ddpm_step (no rescale without CFG, as in the reference). */
+int b200vton_cfg_rescale_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                   const void* noise, const void* coef, int do_cfg, void* out, void* stream);
+
 /* Pre-processing of the inpainting inputs in one launch (diffusers VaeImageProcessor.preprocess for image and mask,
  * the masked image and the latent-resolution mask: src/tryon_pipeline.py:1588-1602, 940-943). image: [B,3,H,W] fp32;
  * mask: [B,mask_channels,H,W] fp32 (1, or 3 = RGB converted to grayscale); image_min: device scalar = min(image)
