@@ -6,21 +6,31 @@
 //     (the reference computes and discards the Ng garment query rows).
 //   * CFG-uncond samples (b < kv1_off) see ZERO garment features (src/tryon_pipeline.py:1796): K=V=0, so each of the N1
 //     tokens adds exp(0 - m) to the softmax denominator and nothing to the numerator. Closed form, no KV traffic.
-//   * attn2 (ip_adapter/attention_processor.py:1943-1995, IPAttnProcessor2_0): the text softmax, then the IP-token softmax
-//     with accumulate = 1 and out_scale = ip_scale: out = fp16(fp16(O_t) + fp16(ip_scale * fp16(O_i))), the reference's
-//     rounding points (cross_attn_impl).
+//   * attn2 (ip_adapter/attention_processor.py:1943-1995, IPAttnProcessor2_0): the text softmax and the IP-token softmax
+//     in one launch (segment 0 = text, segment 1 = IP tokens, flash_kernel<4, true>): out = fp16(fp16(O_t) + fp16(ip_scale * fp16(O_i))),
+//     the reference's rounding points (cross_attn_impl).
 //   * the CLIP towers' encoder self-attention (heads of 64 or 80, optional causal mask; enc_attn_impl).
 //
 // Head dimension D = 16..96 in steps of 16: a head's columns are fetched as R = ceil(D/64) 128B-swizzled regions of 64
 // columns straight out of the projection buffer (the second region runs into the next head's columns, which are never
 // used: Q K^T issues exactly D/16 k-steps and the extra output columns of P V are never stored).
 //
-// One CTA = one (sample, head, 128-query tile): two warpgroups of 64 query rows each. Thread 0 issues the TMA loads (Q once,
-// K/V tiles of 128 keys through a 2-stage ring, the next tile of a stage as soon as both warpgroups have released it); a
-// separate producer warp would cap the consumers at 168 registers and make them spill. Per K/V tile a warpgroup computes
-// S = Q K^T (m64n128k16, both operands in shared memory) into registers, runs the online softmax there (a row lives in
-// the 4 threads of a quad), converts P to fp16 A fragments in registers and accumulates O += P V (m64nDNk16, V as the
-// MN-major B operand).
+// One CTA = one (sample, head, 128-query tile), three warpgroups (FA3 layout):
+//   * warpgroup 2 is the producer: it gives up registers (setmaxnreg.dec) and one thread issues every TMA load: Q once,
+//     then the K/V tiles of 128 keys of segment 0 and segment 1 through a ring of FlashSmem::STAGES stages (3 for D <= 64,
+//     2 above: what 227 KB of shared memory holds);
+//   * warpgroups 0 and 1 are the consumers, 64 query rows each (setmaxnreg.inc). Per K/V tile j a consumer computes
+//     S = Q K_j^T (m64n128k16, both operands in shared memory) into registers, runs the online softmax there (a row lives
+//     in the 4 threads of a quad), converts P to fp16 A fragments in registers and accumulates O += P V_j (m64nDNk16,
+//     V as the MN-major B operand).
+// Overlap: a consumer issues S_{j+1} = Q K_{j+1}^T together with O += P_j V_j and runs the softmax of tile j+1 while
+// P_j V_j is still in the tensor cores (wgmma_wait<1>); and the two consumers issue their MMAs in turns ordered by two
+// named barriers (ping-pong), so one warpgroup's softmax runs while the other's MMAs do. The arithmetic of every
+// element is that of the plain loop (O is rescaled by alpha_j before P_j V_j is added), so the overlap changes no bit.
+// Full key tiles take an unmasked softmax; only the last, partial tile of a segment and causal tiles test each key.
+// Samples with a real segment 1 (b >= kv1_off, the longest CTAs) are scheduled before the zero-K/V samples.
+// With IP (the decoupled text + IP-token cross-attention), segment 1 has its own softmax and the CTA stores
+// fp16(fp16(O_0) + fp16(out_scale * fp16(O_1))).
 #include "common.cuh"
 #include "host.h"
 #include "wgmma.cuh"
@@ -42,15 +52,18 @@ struct FlashParams {
 };
 
 constexpr int FA_REGION = 128 * 128;  // 128 rows x 64 halves
-constexpr int FA_STAGES = 2;
-constexpr int FA_THREADS = 256;       // 2 warpgroups; thread 0 also issues the TMA loads
+constexpr int FA_THREADS = 384;       // consumer warpgroups 0 and 1, producer warpgroup 2
+constexpr int FA_PRODUCER_REGS = 40;  // 128 * 40 + 256 * 232 = 64512 <= 65536 registers per SM
+constexpr int FA_CONSUMER_REGS = 232;
+constexpr uint32_t FA_BAR_TURN = 1;   // named barriers FA_BAR_TURN + wg: consumer wg may issue its MMAs (0 = __syncthreads)
 
 template <int R>
 struct FlashSmem {
+  static constexpr int STAGES = R == 1 ? 3 : 2;
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_K = OFF_Q + R * FA_REGION;
-  static constexpr int OFF_V = OFF_K + FA_STAGES * R * FA_REGION;
-  static constexpr int OFF_BAR = OFF_V + FA_STAGES * R * FA_REGION;
+  static constexpr int OFF_V = OFF_K + STAGES * R * FA_REGION;
+  static constexpr int OFF_BAR = OFF_V + STAGES * R * FA_REGION;
   static constexpr int TOTAL = OFF_BAR + 64 + 1024;
 };
 
@@ -60,27 +73,46 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// KS: Q K^T k-steps (D / 16); R: 64-column regions per head; DN: P V tile width (64 for D <= 64, 96 otherwise)
-template <int KS, int R = (KS + 3) / 4, int DN = (KS <= 4 ? 64 : 96)>
+// KS: Q K^T k-steps (D / 16); IP: segment 1 has a softmax of its own (the text + IP-token cross-attention, D = 64);
+// R: 64-column regions per head; DN: P V tile width (64 for D <= 64, 96 otherwise). D > 64 (the CLIP image tower)
+// and IP do not overlap a warpgroup's softmax with its own P V: S, P and a 96-wide O (or O and the kept fp16 O_0) do not
+// fit the registers together.
+template <int KS, bool IP = false, int R = (KS + 3) / 4, int DN = (KS <= 4 ? 64 : 96)>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
              const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
              const __grid_constant__ CUtensorMap tmV1, const FlashParams p) {
   using SM = FlashSmem<R>;
+  constexpr int ST = SM::STAGES;
+  constexpr bool OVERLAP = DN == 64 && !IP;   // IP runs two tiles, one per softmax: nothing to overlap
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + SM::OFF_BAR;
   const uint32_t q_full = bar_base;
   auto kv_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bar_base + 8u * (1 + FA_STAGES + s); };
+  auto kv_empty = [&](int s) { return bar_base + 8u * (1 + ST + s); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int q_tile = blockIdx.x;
   const int h = blockIdx.y;
-  const int b = blockIdx.z;
+  // heaviest first: the samples that read a segment 1 (b >= kv1_off) get the lowest block indices
+  int b = blockIdx.z;
+  if (p.N1 > 0 && p.kv1_off > 0 && p.kv1_off < p.B) {
+    b += p.kv1_off;
+    if (b >= p.B) b -= p.B;
+  }
 
   if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(kv_full(s), 1);
+      mbar_init(kv_empty(s), 2);   // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  if (threadIdx.x == 256) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK0);
     tma_prefetch_desc(&tmV0);
@@ -88,12 +120,6 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       tma_prefetch_desc(&tmK1);
       tma_prefetch_desc(&tmV1);
     }
-    mbar_init(q_full, 1);
-    for (int s = 0; s < FA_STAGES; ++s) {
-      mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 2);   // one arrival per warpgroup
-    }
-    fence_barrier_init();
   }
   // Programmatic dependent launch: Q/K/V (and kv1_base) are written by the previous kernels of the stream
   pdl_wait();
@@ -111,35 +137,39 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   // causal: key tiles entirely after the last query row of this CTA contribute nothing
   const int total = p.causal ? min(tiles0, q_tile + 1) : tiles0 + tiles1;
 
-  // TMA loads are issued by thread 0: K/V tile j into stage j % FA_STAGES (the stage's previous tile must be released)
-  auto issue_kv = [&](int j) {
-    const int stage = j % FA_STAGES;
-    if (j >= FA_STAGES) mbar_wait(kv_empty(stage), ((j / FA_STAGES) - 1) & 1);
-    mbar_expect_tx(kv_full(stage), 2 * R * FA_REGION);
+  // ===================== producer =====================
+  if (wg == 2) {
+    setmaxnreg_dec<FA_PRODUCER_REGS>();
+    if (threadIdx.x == 256) {
+      mbar_expect_tx(q_full, R * FA_REGION);
 #pragma unroll
-    for (int r = 0; r < R; ++r) {
-      const uint32_t kdst = smem_base + SM::OFF_K + (stage * R + r) * FA_REGION;
-      const uint32_t vdst = smem_base + SM::OFF_V + (stage * R + r) * FA_REGION;
-      const int col = h * p.D + r * 64;
-      if (j < tiles0) {
-        tma_load_3d(kdst, &tmK0, kv_full(stage), col, j * 128, b);
-        tma_load_3d(vdst, &tmV0, kv_full(stage), col, j * 128, b);
-      } else {
-        tma_load_3d(kdst, &tmK1, kv_full(stage), col, (j - tiles0) * 128, idx1);
-        tma_load_3d(vdst, &tmV1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+      for (int r = 0; r < R; ++r)
+        tma_load_3d(smem_base + SM::OFF_Q + r * FA_REGION, &tmQ, q_full, h * p.D + r * 64, q_tile * 128, b);
+      // K/V tile j into stage j % ST, once both consumers have released the stage's previous tile
+      for (int j = 0; j < total; ++j) {
+        const int stage = j % ST;
+        if (j >= ST) mbar_wait(kv_empty(stage), ((j / ST) - 1) & 1);
+        mbar_expect_tx(kv_full(stage), 2 * R * FA_REGION);
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+          const uint32_t kdst = smem_base + SM::OFF_K + (stage * R + r) * FA_REGION;
+          const uint32_t vdst = smem_base + SM::OFF_V + (stage * R + r) * FA_REGION;
+          const int col = h * p.D + r * 64;
+          if (j < tiles0) {
+            tma_load_3d(kdst, &tmK0, kv_full(stage), col, j * 128, b);
+            tma_load_3d(vdst, &tmV0, kv_full(stage), col, j * 128, b);
+          } else {
+            tma_load_3d(kdst, &tmK1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+            tma_load_3d(vdst, &tmV1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+          }
+        }
       }
     }
-  };
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(q_full, R * FA_REGION);
-#pragma unroll
-    for (int r = 0; r < R; ++r)
-      tma_load_3d(smem_base + SM::OFF_Q + r * FA_REGION, &tmQ, q_full, h * p.D + r * 64, q_tile * 128, b);
-    for (int j = 0; j < FA_STAGES && j < total; ++j) issue_kv(j);
+    return;
   }
 
   // ===================== consumers =====================
-  const int wg = warp >> 2;
+  setmaxnreg_inc<FA_CONSUMER_REGS>();
   const int row0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);   // this thread's rows: row0 and row0 + 8 of the tile
   const int qi0 = q_tile * 128 + row0, qi1 = qi0 + 8;
   const int cq = (lane & 3) * 2;                                 // first of this thread's two columns per 8-block
@@ -148,15 +178,15 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   float o[DN / 2];
 #pragma unroll
   for (int i = 0; i < DN / 2; ++i) o[i] = 0.f;
+  uint32_t o_seg0[IP ? DN / 4 : 1];   // IP: the normalised output of segment 0, rounded to fp16 (half2 per register)
+#pragma unroll
+  for (int i = 0; i < (IP ? DN / 4 : 1); ++i) o_seg0[i] = 0u;
+  float s[64];
+  uint32_t pa[8][4];
 
-  mbar_wait(q_full, 0);
   const uint32_t q_src = smem_base + SM::OFF_Q + wg * (64 * 128);
-  for (int j = 0; j < total; ++j) {
-    const int stage = j % FA_STAGES;
-    mbar_wait(kv_full(stage), (j / FA_STAGES) & 1);
+  auto issue_s = [&](int stage) {
     const uint32_t k_src = smem_base + SM::OFF_K + stage * R * FA_REGION;
-    const uint32_t v_src = smem_base + SM::OFF_V + stage * R * FA_REGION;
-    float s[64];
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < KS; ++k) {
@@ -165,24 +195,51 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
                               k > 0 ? 1 : 0);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
-
+  };
+  auto issue_pv = [&](int stage) {
+    const uint32_t v_src = smem_base + SM::OFF_V + stage * R * FA_REGION;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 V rows of 128 B per step
+      WgmmaF16RS<DN>::mma(o, pa[kk], make_gmma_desc_sw128(v_src + kk * 2048, FA_REGION, 1024), 1);
+    wgmma_commit();
+  };
+  // Ping-pong: a consumer issues its MMAs between turn_begin and turn_end. Warpgroup 1 opens warpgroup 0's first turn;
+  // both consumers take the same number of turns, and warpgroup 1's last arrival would have no matching wait, so it is
+  // skipped.
+  auto turn_begin = [&]() { named_bar_sync(FA_BAR_TURN + wg, 256); };
+  auto turn_end = [&](bool last) {
+    if (!(last && wg == 1)) named_bar_arrive(FA_BAR_TURN + (wg ^ 1), 256);
+  };
+  // Online softmax of tile j in s: new row maxima, alpha, P = exp2(s * sl2 - m * sl2) in place, row sums updated
+  auto softmax = [&](int j, float& alpha0, float& alpha1) {
     const int key0 = (j < tiles0) ? j * 128 : (j - tiles0) * 128;
     const int kv_valid = (j < tiles0) ? min(128, p.N0 - key0) : min(128, p.N1 - key0);
+    const bool masked = p.causal || kv_valid < 128;
     float mx0 = -INFINITY, mx1 = -INFINITY;
+    if (masked) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+      for (int i = 0; i < 16; ++i) {
 #pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int col = i * 8 + cq + u;
-        bool ok = col < kv_valid;
-        const bool ok0 = ok && (!p.causal || key0 + col <= qi0);
-        const bool ok1 = ok && (!p.causal || key0 + col <= qi1);
-        if (!ok0) s[4 * i + u] = -INFINITY;
-        if (!ok1) s[4 * i + 2 + u] = -INFINITY;
-        mx0 = fmaxf(mx0, s[4 * i + u]);
-        mx1 = fmaxf(mx1, s[4 * i + 2 + u]);
+        for (int u = 0; u < 2; ++u) {
+          const int col = i * 8 + cq + u;
+          bool ok = col < kv_valid;
+          const bool ok0 = ok && (!p.causal || key0 + col <= qi0);
+          const bool ok1 = ok && (!p.causal || key0 + col <= qi1);
+          if (!ok0) s[4 * i + u] = -INFINITY;
+          if (!ok1) s[4 * i + 2 + u] = -INFINITY;
+          mx0 = fmaxf(mx0, s[4 * i + u]);
+          mx1 = fmaxf(mx1, s[4 * i + 2 + u]);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          mx0 = fmaxf(mx0, s[4 * i + u]);
+          mx1 = fmaxf(mx1, s[4 * i + 2 + u]);
+        }
       }
     }
     mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
@@ -190,35 +247,45 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
     const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
-    const float alpha0 = fast_exp2((m0 - mn0) * sl2), alpha1 = fast_exp2((m1 - mn1) * sl2);
+    alpha0 = fast_exp2((m0 - mn0) * sl2);
+    alpha1 = fast_exp2((m1 - mn1) * sl2);
     const float ms0 = mn0 * sl2, ms1 = mn1 * sl2;
     m0 = mn0;
     m1 = mn1;
     float sum0 = 0.f, sum1 = 0.f;
+    if (masked) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+      for (int i = 0; i < 16; ++i) {
 #pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const float x0 = s[4 * i + u], x1 = s[4 * i + 2 + u];
-        const float p0 = x0 == -INFINITY ? 0.f : fast_exp2(x0 * sl2 - ms0);
-        const float p1 = x1 == -INFINITY ? 0.f : fast_exp2(x1 * sl2 - ms1);
-        s[4 * i + u] = p0;
-        s[4 * i + 2 + u] = p1;
-        sum0 += p0;
-        sum1 += p1;
+        for (int u = 0; u < 2; ++u) {
+          const float x0 = s[4 * i + u], x1 = s[4 * i + 2 + u];
+          const float p0 = x0 == -INFINITY ? 0.f : fast_exp2(x0 * sl2 - ms0);
+          const float p1 = x1 == -INFINITY ? 0.f : fast_exp2(x1 * sl2 - ms1);
+          s[4 * i + u] = p0;
+          s[4 * i + 2 + u] = p1;
+          sum0 += p0;
+          sum1 += p1;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const float p0 = fast_exp2(s[4 * i + u] * sl2 - ms0);
+          const float p1 = fast_exp2(s[4 * i + 2 + u] * sl2 - ms1);
+          s[4 * i + u] = p0;
+          s[4 * i + 2 + u] = p1;
+          sum0 += p0;
+          sum1 += p1;
+        }
       }
     }
     l0 = l0 * alpha0 + sum0;
     l1 = l1 * alpha1 + sum1;
-#pragma unroll
-    for (int i = 0; i < DN / 8; ++i) {
-      o[4 * i] *= alpha0;
-      o[4 * i + 1] *= alpha0;
-      o[4 * i + 2] *= alpha1;
-      o[4 * i + 3] *= alpha1;
-    }
-    // P (fp16, unnormalised, <= 1) as the A fragments of the 8 k-steps of 16 keys
-    uint32_t pa[8][4];
+  };
+  // P (fp16, unnormalised, <= 1) as the A fragments of the 8 k-steps of 16 keys
+  auto pack_p = [&]() {
 #pragma unroll
     for (int kk = 0; kk < 8; ++kk) {
       pa[kk][0] = pack_h2(s[8 * kk + 0], s[8 * kk + 1]);
@@ -226,16 +293,111 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       pa[kk][2] = pack_h2(s[8 * kk + 4], s[8 * kk + 5]);
       pa[kk][3] = pack_h2(s[8 * kk + 6], s[8 * kk + 7]);
     }
-    fence_regs(o);
-    wgmma_fence();
+  };
+
+  auto rescale_o = [&](float alpha0, float alpha1) {
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 V rows of 128 B per step
-      WgmmaF16RS<DN>::mma(o, pa[kk], make_gmma_desc_sw128(v_src + kk * 2048, FA_REGION, 1024), 1);
-    wgmma_commit();
+    for (int i = 0; i < DN / 8; ++i) {
+      o[4 * i] *= alpha0;
+      o[4 * i + 1] *= alpha0;
+      o[4 * i + 2] *= alpha1;
+      o[4 * i + 3] *= alpha1;
+    }
+  };
+  // IP: at the first tile of segment 1, keep fp16(O_0 / l_0) and restart the softmax (called after softmax(j) with the
+  // segment-0 row sums saved in ls0 / ls1)
+  auto close_segment0 = [&](float ls0, float ls1) {
+    ls0 += __shfl_xor_sync(0xffffffffu, ls0, 1);
+    ls0 += __shfl_xor_sync(0xffffffffu, ls0, 2);
+    ls1 += __shfl_xor_sync(0xffffffffu, ls1, 1);
+    ls1 += __shfl_xor_sync(0xffffffffu, ls1, 2);
+    const float i0 = 1.f / ls0, i1 = 1.f / ls1;
+#pragma unroll
+    for (int i = 0; i < DN / 8; ++i) {
+      if constexpr (IP) {
+        o_seg0[2 * i] = pack_h2(o[4 * i] * i0, o[4 * i + 1] * i0);
+        o_seg0[2 * i + 1] = pack_h2(o[4 * i + 2] * i1, o[4 * i + 3] * i1);
+      }
+      o[4 * i] = o[4 * i + 1] = o[4 * i + 2] = o[4 * i + 3] = 0.f;
+    }
+  };
+
+  if (wg == 1) named_bar_arrive(FA_BAR_TURN, 256);
+  mbar_wait(q_full, 0);
+  if constexpr (OVERLAP) {
+    // tile 0: S_0 alone (O is still zero, so no rescale)
+    mbar_wait(kv_full(0), 0);
+    turn_begin();
+    issue_s(0);
+    turn_end(false);
+    wgmma_wait<0>();
+    fence_regs(s);
+    {
+      float a0, a1;
+      softmax(0, a0, a1);
+    }
+    pack_p();
+    for (int j = 1; j < total; ++j) {
+      const int stage = j % ST, prev = (j - 1) % ST;
+      mbar_wait(kv_full(stage), (j / ST) & 1);
+      turn_begin();
+      issue_s(stage);
+      issue_pv(prev);
+      turn_end(false);
+      wgmma_wait<1>();   // S_j is in registers; P_{j-1} V_{j-1} may still run
+      fence_regs(s);
+      const bool seg_start = IP && j == tiles0;
+      float ls0 = l0, ls1 = l1;
+      if (seg_start) {   // the IP tokens' softmax starts afresh
+        m0 = m1 = -INFINITY;
+        l0 = l1 = 0.f;
+      }
+      float alpha0, alpha1;
+      softmax(j, alpha0, alpha1);
+      wgmma_wait<0>();
+      fence_regs(o);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty(prev));
+      if (seg_start)
+        close_segment0(ls0, ls1);
+      else
+        rescale_o(alpha0, alpha1);
+      pack_p();
+    }
+    turn_begin();
+    issue_pv((total - 1) % ST);
+    turn_end(true);
     wgmma_wait<0>();
     fence_regs(o);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty(stage));
-    if (threadIdx.x == 0 && j + FA_STAGES < total) issue_kv(j + FA_STAGES);
+  } else {
+    for (int j = 0; j < total; ++j) {
+      const int stage = j % ST;
+      mbar_wait(kv_full(stage), (j / ST) & 1);
+      turn_begin();
+      issue_s(stage);
+      turn_end(false);
+      wgmma_wait<0>();
+      fence_regs(s);
+      const bool seg_start = IP && j == tiles0;
+      float ls0 = l0, ls1 = l1;
+      if (seg_start) {
+        m0 = m1 = -INFINITY;
+        l0 = l1 = 0.f;
+      }
+      float alpha0, alpha1;
+      softmax(j, alpha0, alpha1);
+      if (seg_start)
+        close_segment0(ls0, ls1);
+      else
+        rescale_o(alpha0, alpha1);
+      pack_p();
+      fence_regs(o);
+      turn_begin();
+      issue_pv(stage);
+      turn_end(j == total - 1);
+      wgmma_wait<0>();
+      fence_regs(o);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty(stage));
+    }
   }
 
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
@@ -258,6 +420,7 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   }
   const float inv[2] = {1.f / l0, 1.f / l1};
   const int qi[2] = {qi0, qi1};
+  const bool two_softmax = IP && tiles1 > 0;
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     if (qi[hr] >= p.Nq) continue;
@@ -267,7 +430,11 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       const int col = i * 8 + cq;
       if (col >= p.D) continue;
       float v0 = o[4 * i + 2 * hr] * inv[hr], v1 = o[4 * i + 2 * hr + 1] * inv[hr];
-      if (p.accumulate) {
+      if (two_softmax) {
+        const float2 t = unpack_h2(o_seg0[IP ? 2 * i + hr : 0]);
+        v0 = t.x + round_h(p.out_scale * round_h(v0));
+        v1 = t.y + round_h(p.out_scale * round_h(v1));
+      } else if (p.accumulate) {
         const float2 a = unpack_h2(*reinterpret_cast<const uint32_t*>(dst + col));
         v0 = a.x + round_h(p.out_scale * round_h(v0));
         v1 = a.y + round_h(p.out_scale * round_h(v1));
@@ -277,8 +444,9 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   }
 }
 
-// Tuning switches of other attention kernels of this library's C ABI; there is one attention kernel here, so the options
-// "attention_pingpong", "attention_q_tiles" and "attention_poly_exp" are accepted and have no effect.
+// Tuning switches of other attention kernels of this library's C ABI. There is one attention kernel here, which always
+// runs the ping-pong schedule with 128-query tiles and ex2.approx, so the options "attention_pingpong",
+// "attention_q_tiles" and "attention_poly_exp" are accepted and have no effect.
 void set_attn_poly(int) {}
 void set_attn_qtiles(int) {}
 void set_attn_v2(int) {}
@@ -290,11 +458,11 @@ static int encode_tokens(CUtensorMap* tm, const void* base, long long ld, int co
   return encode_tmap_f16(tm, base, 3, dims, strides, box);
 }
 
-template <int KS>
+template <int KS, bool IP = false>
 static int launch_flash(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const CUtensorMap& tmV0, const CUtensorMap& tmK1,
                         const CUtensorMap& tmV1, const FlashParams& p, cudaStream_t stream) {
   constexpr int R = (KS + 3) / 4;
-  auto kern = flash_kernel<KS>;
+  auto kern = flash_kernel<KS, IP>;
   static bool configured = false;
   if (!configured) {
     VTON_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FlashSmem<R>::TOTAL));
@@ -307,8 +475,10 @@ static int launch_flash(const CUtensorMap& tmQ, const CUtensorMap& tmK0, const C
 }
 
 // One launch: q [B, Nq, >= H*D] (row stride ldq); k0/v0 [B, N0, .] (ldkv0); k1/v1 [B1, N1, .] (ldkv1) or null.
+// ip: segment 1 is the IP tokens of the decoupled cross-attention (D = 64), with a softmax of its own.
 static int flash(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
-                 const void* v1, long long ldkv1, int B1, void* out, long long ldo, FlashParams p, cudaStream_t stream) {
+                 const void* v1, long long ldkv1, int B1, void* out, long long ldo, FlashParams p, cudaStream_t stream,
+                 bool ip = false) {
   CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
   const int cols = p.H * p.D;
   if (int e = encode_tokens(&tmQ, q, ldq, cols, p.Nq, p.B)) return e;
@@ -322,6 +492,7 @@ static int flash(const void* q, long long ldq, const void* k0, const void* v0, l
   }
   p.out = static_cast<__half*>(out);
   p.ld_out = static_cast<int>(ldo);
+  if (ip) return launch_flash<4, true>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
   switch (p.D / 16) {
     case 1: return launch_flash<1>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
     case 2: return launch_flash<2>(tmQ, tmK0, tmV0, tmK1, tmV1, p, stream);
@@ -376,21 +547,20 @@ int cross_attn_impl(const void* q, long long ldq, const void* kt, const void* vt
                  "cross_attn: row strides must be multiples of 8");
   VTON_CHECK_ARG(aligned_to(out, 4), "cross_attn: out must be 4-byte aligned (stored two halves at a time)");
   VTON_CHECK_ARG(B <= 65535 && H <= 65535, "cross_attn: grid too large");
+  // one launch: Q is read once, segment 0 = the text tokens, segment 1 = the IP tokens of the same sample (kv1_off = 0,
+  // kv1_count = B) with a softmax of its own
   FlashParams p{};
   p.B = B;
   p.H = H;
   p.Nq = Nq;
   p.N0 = Nt;
+  p.N1 = Ni;
   p.D = 64;
-  p.kv1_count = 1;
+  p.kv1_count = B;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.out_scale = 1.f;
-  if (int e = flash(q, ldq, kt, vt, ldkv_t, nullptr, nullptr, 0, 0, out, ldo, p, stream)) return e;
-  if (Ni == 0) return kOk;
-  p.N0 = Ni;
-  p.accumulate = 1;
-  p.out_scale = ip_scale;
-  return flash(q, ldq, ki, vi, ldkv_i, nullptr, nullptr, 0, 0, out, ldo, p, stream);
+  p.out_scale = Ni > 0 ? ip_scale : 1.f;
+  return flash(q, ldq, kt, vt, ldkv_t, Ni > 0 ? ki : nullptr, Ni > 0 ? vi : nullptr, ldkv_i, B, out, ldo, p, stream,
+               Ni > 0);
 }
 
 // Encoder self-attention of the CLIP towers around the denoising loop: the ViT-H image encoder (16 heads of 80, 257

@@ -136,6 +136,16 @@ __device__ __forceinline__ uint64_t make_gmma_desc_sw128(uint32_t saddr, uint32_
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// Warp-specialised kernels: hand registers from the producer warpgroup to the consumers (every warp of the warpgroup
+// executes it; N is a multiple of 8 in [24, 256])
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ----------------------------------------------------------------------------------------------
 // small numeric helpers (fp16 rounding points follow the reference's autocast path)

@@ -1,5 +1,6 @@
 """Per-kernel timing of the hot ops at BASELINE config-2 shapes (device events, L2 flushed between launches).
-Prints one line per (op, shape, variant) with achieved TFLOP/s or GB/s. Not a bench value; a tuning aid."""
+Prints one line per (op, shape, variant) with achieved TFLOP/s or GB/s. Not a bench value; a tuning aid.
+MB_ONLY=gemm stops after the GEMM / convolution rows, MB_ONLY=attention runs the attention rows only."""
 import json
 import os
 import sys
@@ -78,7 +79,8 @@ def rec(name, ms, flops=None, bytes_=None, **kw):
 def main():
     L.load()
     # ---- linears (M = 2B*N tokens with B=2: L1 M=12288 C=640, L2 M=3072 C=1280)
-    for (M, N, K, tag) in [(12288, 1920, 640, "L1 qkv"), (12288, 640, 640, "L1 out"), (12288, 5120, 640, "L1 ff1"),
+    skip = ONLY == "attention"
+    for (M, N, K, tag) in [] if skip else [(12288, 1920, 640, "L1 qkv"), (12288, 640, 640, "L1 out"), (12288, 5120, 640, "L1 ff1"),
                            (12288, 640, 2560, "L1 ff2"), (3072, 3840, 1280, "L2 qkv"), (3072, 1280, 1280, "L2 out"),
                            (3072, 10240, 1280, "L2 ff1"), (3072, 1280, 5120, "L2 ff2"), (1536, 2560, 1280, "L2 garment kv"),
                            (8192, 8192, 8192, "square 8k")]:
@@ -104,7 +106,7 @@ def main():
         ref = timeit(lambda: torch.matmul(a, w.t()))
         rec("cublas", ref, flops=2.0 * M * N * K, shape=[M, N, K], tag=tag)
     # ---- convs (NHWC, B=4)
-    for (B, H, W, Cin, Cout, tag) in [(4, 128, 96, 320, 320, "L0 res"), (4, 64, 48, 640, 640, "L1 res"),
+    for (B, H, W, Cin, Cout, tag) in [] if skip else [(4, 128, 96, 320, 320, "L0 res"), (4, 64, 48, 640, 640, "L1 res"),
                                       (4, 32, 24, 1280, 1280, "L2 res"), (4, 32, 24, 2560, 1280, "L2 up res"),
                                       (4, 128, 96, 960, 320, "L0 up res"), (4, 128, 96, 64, 320, "conv_in")]:
         x = rnd(B, H, W, Cin)
@@ -143,6 +145,14 @@ def main():
             ms = timeit(lambda: L.attention(q, k, v, heads=H))
             fl = 4.0 * B * H * N * T * 64
         rec("attention", ms, flops=fl, shape=[B, H, N, Ng], tag=tag)
+    # text (77 tokens) + IP (16 tokens) cross-attention of the try-on blocks, one call
+    for (B, H, N, tag) in [(4, 10, 3072, "L1 cross text+ip"), (4, 20, 768, "L2 cross text+ip")]:
+        C = H * 64
+        q, kt, vt, ki, vi = rnd(B, N, C), rnd(B, 77, C), rnd(B, 77, C), rnd(B, 16, C), rnd(B, 16, C)
+        ms = timeit(lambda: L.cross_attention(q, kt, vt, ki, vi, heads=H))
+        rec("cross_attention", ms, flops=4.0 * B * H * N * (77 + 16) * 64, shape=[B, H, N, 77, 16], tag=tag)
+    if ONLY == "attention":
+        return
     # ---- HBM-bound side kernels
     for (B, HW, C, tag) in [(4, 12288, 320, "L0"), (4, 3072, 640, "L1"), (4, 768, 2560, "L2 cat")]:
         x = rnd(B, HW, C)
