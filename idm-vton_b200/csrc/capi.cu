@@ -29,7 +29,7 @@ int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW
 int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
                    void* out, long long ldo, cudaStream_t stream);
 int nchw_to_nhwc_impl(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
-                      cudaStream_t stream);
+                      const void* scale, cudaStream_t stream);
 int nhwc_to_nchw_impl(const void* src, int B, int C, int H, int W, int ldc, void* dst, cudaStream_t stream);
 int upsample2x_impl(const void* src, int B, int H, int W, int C, void* dst, cudaStream_t stream);
 int im2col_s2_impl(const void* src, int B, int H, int W, int C, void* dst, cudaStream_t stream);
@@ -54,13 +54,15 @@ int cfg_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const vo
                   const void* coef, int do_cfg, void* out, cudaStream_t stream);
 int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
                           const void* coef, int do_cfg, void* out, cudaStream_t stream);
+int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                    void* x0_prev, const void* coef, int kind, int do_cfg, void* out, cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
 
 extern "C" {
 
-int b200vton_version(void) { return 107; }
+int b200vton_version(void) { return 108; }
 const char* b200vton_last_error(void) { return vton::get_last_error(); }
 long long b200vton_launch_count(void) { return vton::launch_count(); }
 int b200vton_set_option(const char* name, int value) {
@@ -167,7 +169,12 @@ int b200vton_layernorm(const void* x, int64_t ldx, int rows, int C, const void* 
 
 int b200vton_nchw_to_nhwc(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
                           void* stream) {
-  return vton::nchw_to_nhwc_impl(src, Bs, Cs, H, W, dst, Bd, ldc, c_off, S(stream));
+  return vton::nchw_to_nhwc_impl(src, Bs, Cs, H, W, dst, Bd, ldc, c_off, nullptr, S(stream));
+}
+int b200vton_nchw_to_nhwc_scaled(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
+                                 const void* scale, void* stream) {
+  VTON_CHECK_ARG(scale, "nchw_to_nhwc_scaled: scale is null");
+  return vton::nchw_to_nhwc_impl(src, Bs, Cs, H, W, dst, Bd, ldc, c_off, scale, S(stream));
 }
 int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, void* dst, void* stream) {
   return vton::nhwc_to_nchw_impl(src, B, C, H, W, ldc, dst, S(stream));
@@ -194,6 +201,11 @@ int b200vton_cfg_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W,
 int b200vton_cfg_rescale_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
                                    const void* noise, const void* coef, int do_cfg, void* out, void* stream) {
   return vton::cfg_rescale_ddpm_impl(eps, ldc, B, C, H, W, latents, noise, coef, do_cfg, out, S(stream));
+}
+int b200vton_cfg_solver_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                             const void* noise, void* x0_prev, const void* coef, int kind, int do_cfg, void* out,
+                             void* stream) {
+  return vton::cfg_solver_impl(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, kind, do_cfg, out, S(stream));
 }
 
 int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_channels, const void* image_min, int B,

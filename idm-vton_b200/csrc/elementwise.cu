@@ -11,14 +11,24 @@ namespace vton {
 // scatter: dst[s, y, x, c_off + c] = src[s % Bs, c, y, x]   (CFG duplication `torch.cat([latents]*2)`,
 //          src/tryon_pipeline.py:1769, and the 13-channel concat, :1777, become channel offsets)
 // ------------------------------------------------------------------------------------------------
-__global__ void nchw_to_nhwc_kernel(const __half* src, int Bs, int Cs, int HW, __half* dst, int Bd, int ldc, int c_off) {
+// scale (device scalar, may be null): dst = fp16(src * scale[0]) instead of a copy. This is the
+// `scheduler.scale_model_input` of EulerDiscreteScheduler (src/tryon_pipeline.py:1772): the caller passes the fp32
+// reciprocal 1 / sqrt(sigma^2 + 1), because torch divides a CUDA tensor by a CPU scalar as a product with its reciprocal.
+__global__ void nchw_to_nhwc_kernel(const __half* src, int Bs, int Cs, int HW, __half* dst, int Bd, int ldc, int c_off,
+                                    const float* scale) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(Bd) * HW;
   if (i >= total) return;
   const int s = static_cast<int>(i / HW);
   const int px = static_cast<int>(i % HW);
   const int sb = s % Bs;
-  for (int c = 0; c < Cs; ++c) dst[i * ldc + c_off + c] = src[(static_cast<long long>(sb) * Cs + c) * HW + px];
+  if (scale) {
+    const float f = *scale;
+    for (int c = 0; c < Cs; ++c)
+      dst[i * ldc + c_off + c] = f2h(h2f(src[(static_cast<long long>(sb) * Cs + c) * HW + px]) * f);
+  } else {
+    for (int c = 0; c < Cs; ++c) dst[i * ldc + c_off + c] = src[(static_cast<long long>(sb) * Cs + c) * HW + px];
+  }
 }
 
 __global__ void nhwc_to_nchw_kernel(const __half* src, int B, int C, int HW, int ldc, __half* dst) {
@@ -32,11 +42,13 @@ __global__ void nhwc_to_nchw_kernel(const __half* src, int B, int C, int HW, int
 }
 
 int nchw_to_nhwc_impl(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
-                      cudaStream_t stream) {
+                      const void* scale, cudaStream_t stream) {
   VTON_CHECK_ARG(Bs > 0 && Cs > 0 && H > 0 && W > 0 && Bd > 0 && c_off + Cs <= ldc, "nchw_to_nhwc: bad shape");
+  VTON_CHECK_ARG(aligned_to(scale, 4), "nchw_to_nhwc: scale must be 4-byte aligned");
   const long long total = static_cast<long long>(Bd) * H * W;
   nchw_to_nhwc_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
-      static_cast<const __half*>(src), Bs, Cs, H * W, static_cast<__half*>(dst), Bd, ldc, c_off);
+      static_cast<const __half*>(src), Bs, Cs, H * W, static_cast<__half*>(dst), Bd, ldc, c_off,
+      static_cast<const float*>(scale));
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;
@@ -361,6 +373,92 @@ int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, 
   cfg_rescale_ddpm_kernel<<<B, kRescaleThreads, 0, stream>>>(
       static_cast<const __half*>(eps), ldc, B, C, H * W, static_cast<const __half*>(latents),
       static_cast<const __half*>(noise), static_cast<const float*>(coef), static_cast<__half*>(out));
+  count_launch();
+  VTON_CUDA(cudaGetLastError());
+  return kOk;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Fused CFG + one step of DDIM, Euler or DPM-Solver++ (src/tryon_pipeline.py:1814-1823 with a DDIMScheduler,
+// EulerDiscreteScheduler or DPMSolverMultistepScheduler, epsilon prediction). Same layout as cfg_ddpm_kernel, plus
+// x0_prev: the previous step's data prediction [B,C,H,W] fp16 (DPM-Solver++ only; read, then overwritten with this
+// step's). coef: 8 fp32 on the device {gs, s, inv_a, p, q, r, sigma_n, k}. In exact arithmetic every kind is
+//   g = CFG(eps);  x0 = (x - s g) / a;  D = (1 + k/2) x0 - (k/2) x0_prev;  out = p x + q D + r g + sigma_n noise
+// and the kinds differ in their rounding points, which are those of the scheduler's own `step` on fp16 tensors
+// (g = u + fp16(gs * fp16(t - u)) under CFG for all three; a CPU-scalar divisor is a product with its fp32 reciprocal):
+//   DDIM   (kind 0, fp16 tensor arithmetic; p and k unused):
+//          x0 = fp16(fp16(x - fp16(s g)) * inv_a);  out = fp16(fp16(q x0) + fp16(r g));
+//          out = fp16(out + fp16(sigma_n noise))                      (eta > 0 only)
+//   Euler  (kind 1, sample upcast to fp32; s = sigma, inv_a = 1 / sigma, r = sigma_next - sigma; p, q, k unused):
+//          x0 = x - fp16(s g);  d = (x - x0) * inv_a;  out = fp16(x + d r)           (fp32 ops, no FMA contraction)
+//   DPM++  (kind 2, data prediction in fp16, update with the sample in fp32; s = sigma_t, inv_a = 1 / alpha_t of the
+//          solver at this step, p = sigma_next / sigma_t, q = alpha_next (1 - e^-h), k = 1 / r0 at second order and 0
+//          at first order; r unused):
+//          x0 = fp16(fp16(x - fp16(s g)) * inv_a);
+//          out = fp16((p x + fp16(q x0)) + fp16(fp32(q / 2) * fp16(k * fp16(x0 - x0_prev))));  x0_prev = x0
+// sigma_n * noise is added the same way by every kind when noise is not null (only DDIM with eta > 0 draws it).
+// ------------------------------------------------------------------------------------------------
+template <int KIND>
+__global__ void cfg_solver_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents,
+                                  const __half* noise, __half* x0_prev, const float* coef, int do_cfg, __half* out) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long total = static_cast<long long>(B) * C * HW;
+  if (i >= total) return;
+  const int px = static_cast<int>(i % HW);
+  const int c = static_cast<int>((i / HW) % C);
+  const int b = static_cast<int>(i / (static_cast<long long>(HW) * C));
+  const float gs = coef[0], s = coef[1], inv_a = coef[2], p = coef[3], q = coef[4], r = coef[5], sigma_n = coef[6],
+              k = coef[7];
+  float g;
+  if (do_cfg) {
+    const float u = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
+    const float t = h2f(eps[(static_cast<long long>(b + B) * HW + px) * ldc + c]);
+    g = round_h(u + round_h(gs * round_h(t - u)));
+  } else {
+    g = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
+  }
+  const float x = h2f(latents[i]);
+  float prev;
+  if constexpr (KIND == 0) {
+    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
+    prev = round_h(round_h(q * x0) + round_h(r * g));
+  } else if constexpr (KIND == 1) {
+    const float x0 = __fsub_rn(x, round_h(s * g));
+    const float d = __fmul_rn(__fsub_rn(x, x0), inv_a);
+    prev = round_h(__fadd_rn(x, __fmul_rn(d, r)));
+  } else {
+    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
+    const float d1 = round_h(k * round_h(x0 - h2f(x0_prev[i])));
+    prev = round_h(__fadd_rn(__fadd_rn(__fmul_rn(p, x), round_h(q * x0)), round_h(0.5f * q * d1)));
+    x0_prev[i] = f2h(x0);
+  }
+  if (noise) prev = round_h(prev + round_h(sigma_n * h2f(noise[i])));
+  out[i] = f2h(prev);
+}
+
+int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                    void* x0_prev, const void* coef, int kind, int do_cfg, void* out, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef && eps && latents && out,
+                 "cfg_solver: bad arguments");
+  VTON_CHECK_ARG(kind >= 0 && kind <= 2, "cfg_solver: kind %d is not 0 (DDIM), 1 (Euler) or 2 (DPM-Solver++)", kind);
+  VTON_CHECK_ARG(kind != 2 || x0_prev, "cfg_solver: DPM-Solver++ needs the x0_prev state buffer");
+  VTON_CHECK_ARG(aligned_to(eps, 2) && aligned_to(latents, 2) && aligned_to(noise, 2) && aligned_to(x0_prev, 2) &&
+                     aligned_to(out, 2) && aligned_to(coef, 4),
+                 "cfg_solver: fp16 operands must be 2-byte aligned and coef 4-byte aligned");
+  const long long total = static_cast<long long>(B) * C * H * W;
+  const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+  auto e = static_cast<const __half*>(eps);
+  auto l = static_cast<const __half*>(latents);
+  auto n = static_cast<const __half*>(noise);
+  auto x0p = static_cast<__half*>(x0_prev);
+  auto cf = static_cast<const float*>(coef);
+  auto o = static_cast<__half*>(out);
+  if (kind == 0)
+    cfg_solver_kernel<0><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, do_cfg, o);
+  else if (kind == 1)
+    cfg_solver_kernel<1><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, do_cfg, o);
+  else
+    cfg_solver_kernel<2><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, x0p, cf, do_cfg, o);
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;

@@ -3,7 +3,8 @@
 Per step the reference runs the garment UNet (batch Bg), zero-pads its 70 features for the CFG-uncond half, runs the
 try-on UNet (batch 2B), applies CFG and the DDPM update. Here one step is a fixed launch sequence over static buffers:
   latents -> [NCHW->NHWC scatter into the 13(+pad)-channel input] -> garment UNet -> try-on UNet (garment K/V streamed
-  as a second attention segment, uncond half in closed form) -> fused CFG(+guidance rescale)+DDPM
+  as a second attention segment, uncond half in closed form) -> fused CFG(+guidance rescale)+DDPM, or fused CFG +
+  DDIM / Euler / DPM-Solver++ step (Euler scales the latents in the scatter)
 captured once in a CUDA graph and replayed per step; step-invariant work (cross-attention K/V of text / IP tokens,
 aug_emb, the static input channels) is hoisted to prepare().
 """
@@ -23,6 +24,141 @@ class nvtx_range:
 
     def __exit__(self, *a):
         torch.cuda.nvtx.range_pop()
+
+
+_KINDS = {"DDPMScheduler": "ddpm", "DDIMScheduler": "ddim", "EulerDiscreteScheduler": "euler",
+          "DPMSolverMultistepScheduler": "dpmpp"}
+
+
+def scheduler_kind(scheduler):
+    """"ddpm" | "ddim" | "euler" | "dpmpp": the fused step that implements `scheduler`, from the class names of its
+    type (so a caller's own diffusers scheduler, or a subclass of one, is recognised). An object whose class is not a
+    `...Scheduler` (a bare object carrying the DDPM attributes) is treated as DDPM; every other scheduler class
+    raises NotImplementedError instead of being stepped with the wrong update."""
+    for c in type(scheduler).__mro__:
+        if c.__name__ in _KINDS:
+            return _KINDS[c.__name__]
+    name = type(scheduler).__name__
+    if name.endswith("Scheduler"):
+        raise NotImplementedError(
+            f"{name} is not supported by the engine: its fused step implements DDPMScheduler, DDIMScheduler, "
+            "EulerDiscreteScheduler (s_churn = 0) and DPMSolverMultistepScheduler (dpmsolver++, midpoint, order <= 2)")
+    return "ddpm"
+
+
+def _config_getter(scheduler):
+    cfg = getattr(scheduler, "config", None)
+    return (lambda k, d=None: cfg.get(k, d)) if isinstance(cfg, dict) else (lambda k, d=None: getattr(cfg, k, d))
+
+
+def ddim_step_coefficients(scheduler, t, eta=0.0):
+    """(s, inv_a, p, q, r, sigma_n, k) of DDIMScheduler.step at timestep t (the coefficient layout of
+    b200vton_cfg_solver_step), computed in fp32 torch like diffusers 0.25 from the generic attributes:
+    `alphas_cumprod`, `final_alpha_cumprod` (or `config.set_alpha_to_one`), `config.num_train_timesteps` and
+    `num_inference_steps`. The step goes to t - T_train // num_inference_steps."""
+    get = _config_getter(scheduler)
+    if get("prediction_type", "epsilon") != "epsilon" or get("clip_sample", False) or get("thresholding", False):
+        raise NotImplementedError("the fused DDIM step covers epsilon prediction without clip_sample / thresholding")
+    ac = scheduler.alphas_cumprod.to(device="cpu", dtype=torch.float32)
+    t = int(t)
+    prev_t = t - int(get("num_train_timesteps", len(ac))) // int(scheduler.num_inference_steps)
+    final = getattr(scheduler, "final_alpha_cumprod", None)
+    if final is None:
+        final = torch.tensor(1.0) if get("set_alpha_to_one", True) else ac[0]
+    a_t = ac[t]
+    a_prev = ac[prev_t] if prev_t >= 0 else torch.as_tensor(final, dtype=torch.float32).cpu()
+    var = (1 - a_prev) / (1 - a_t) * (1 - a_t / a_prev)
+    std = eta * var ** 0.5
+    inv_a = torch.tensor(1.0, dtype=torch.float32) / (a_t ** 0.5)
+    return (float((1 - a_t) ** 0.5), float(inv_a), 0.0, float(a_prev ** 0.5), float((1 - a_prev - std ** 2) ** 0.5),
+            float(std), 0.0)
+
+
+def _run_indices(scheduler, timesteps):
+    """Positions in `scheduler.timesteps` of the timesteps a run steps through: the first found like diffusers'
+    `_init_step_index` (the second match when it occurs twice), then one further per step."""
+    sched = scheduler.timesteps.detach().cpu().to(torch.float64)
+    run = [float(t) for t in timesteps]
+    idx = (sched == run[0]).nonzero().flatten().tolist()
+    if not idx:
+        raise ValueError(f"timestep {run[0]} is not in {type(scheduler).__name__}.timesteps")
+    start = idx[1] if len(idx) > 1 else idx[0]
+    if sched[start:start + len(run)].tolist() != run:
+        raise ValueError("the run's timesteps must be consecutive entries of the scheduler's timesteps")
+    return list(range(start, start + len(run)))
+
+
+def euler_step_tables(scheduler, timesteps):
+    """([(s, inv_a, p, q, r, sigma_n, k)], [input scale]) per step of EulerDiscreteScheduler at s_churn = 0 (the
+    pipeline passes no s_churn), in fp32 torch like diffusers 0.25, from `sigmas` (N + 1 values) and `timesteps`."""
+    get = _config_getter(scheduler)
+    if get("prediction_type", "epsilon") != "epsilon" or get("interpolation_type", "linear") != "linear":
+        raise NotImplementedError("the fused Euler step covers epsilon prediction with linear sigma interpolation")
+    sig = scheduler.sigmas.detach().to(device="cpu", dtype=torch.float32)
+    rows, scales = [], []
+    for i in _run_indices(scheduler, timesteps):
+        sigma, sigma_next = sig[i], sig[i + 1]
+        rows.append((float(sigma), float(torch.tensor(1.0) / sigma), 1.0, 0.0, float(sigma_next - sigma), 0.0, 0.0))
+        scales.append(float(torch.tensor(1.0) / ((sigma ** 2 + 1) ** 0.5)))
+    return rows, scales
+
+
+def dpmpp_step_coefficients_table(scheduler, timesteps):
+    """[(s, inv_a, p, q, r, sigma_n, k)] per step of DPMSolverMultistepScheduler (dpmsolver++, midpoint, order 1 / 2),
+    in fp32 torch like diffusers 0.25, from `sigmas`, `timesteps` and the config's solver_order, lower_order_final and
+    euler_at_final; k = 1 / r0 at second-order steps and 0 at first-order ones."""
+    from .scheduler import solver_order_at
+    get = _config_getter(scheduler)
+    if get("solver_order", 2) not in (1, 2):
+        raise NotImplementedError(f"solver_order {get('solver_order')}: the fused DPM-Solver++ step covers orders 1 and 2")
+    if get("algorithm_type", "dpmsolver++") != "dpmsolver++":
+        raise NotImplementedError(f"algorithm_type {get('algorithm_type')}: the fused step covers dpmsolver++ only")
+    if get("solver_type", "midpoint") != "midpoint":
+        raise NotImplementedError(f"solver_type {get('solver_type')}: the fused step covers midpoint only")
+    if get("thresholding", False) or get("prediction_type", "epsilon") != "epsilon" or get("use_lu_lambdas", False):
+        raise NotImplementedError("the fused DPM-Solver++ step covers epsilon prediction without thresholding or "
+                                  "use_lu_lambdas")
+    sig = scheduler.sigmas.detach().to(device="cpu", dtype=torch.float32)
+    n = len(scheduler.timesteps)
+
+    def alpha_sigma(i):
+        alpha = 1 / ((sig[i] ** 2 + 1) ** 0.5)
+        return alpha, sig[i] * alpha
+
+    rows = []
+    for j, i in enumerate(_run_indices(scheduler, timesteps)):
+        alpha_t, sigma_t = alpha_sigma(i)
+        alpha_n, sigma_n = alpha_sigma(i + 1)
+        lam = torch.log(alpha_t) - torch.log(sigma_t)
+        h = torch.log(alpha_n) - torch.log(sigma_n) - lam
+        c = alpha_n * (torch.exp(-h) - 1.0)
+        k = 0.0
+        if solver_order_at(j, i, n, scheduler.config) == 2:
+            alpha_p, sigma_p = alpha_sigma(i - 1)
+            r0 = (lam - (torch.log(alpha_p) - torch.log(sigma_p))) / h
+            k = float(1.0 / r0)
+        rows.append((float(sigma_t), float(torch.tensor(1.0) / alpha_t), float(sigma_n / sigma_t), float(-c), 0.0, 0.0, k))
+    return rows
+
+
+def solver_step_tables(scheduler, timesteps, eta=0.0):
+    """The per-step tables of the fused step for `scheduler` over the run's `timesteps`:
+    (kind, rows, scales, draws, noise_applied). rows: the kernel's coefficients after the guidance scale (5 DDPM values
+    for "ddpm", the 7 of b200vton_cfg_solver_step otherwise); scales: the input scale of each step (Euler's
+    scale_model_input, else None); draws: whether the scheduler's own `step` draws a variance-noise tensor from the
+    generator at that step (DDPM at t > 0, DDIM at eta > 0, Euler at every step); noise_applied: whether that draw enters
+    the update (Euler draws it and multiplies it by zero at s_churn = 0)."""
+    kind = scheduler_kind(scheduler)
+    T = len(timesteps)
+    if kind == "ddpm":
+        return kind, [ddpm_step_coefficients(scheduler, int(t)) for t in timesteps], None, \
+            [int(t) > 0 for t in timesteps], True
+    if kind == "ddim":
+        return kind, [ddim_step_coefficients(scheduler, t, eta) for t in timesteps], None, [eta > 0] * T, True
+    if kind == "euler":
+        rows, scales = euler_step_tables(scheduler, timesteps)
+        return kind, rows, scales, [True] * T, False
+    return kind, dpmpp_step_coefficients_table(scheduler, timesteps), None, [False] * T, False
 
 
 def ddpm_step_coefficients(scheduler, t):
@@ -170,7 +306,9 @@ class TryOnDenoiser:
             self.x_t = torch.zeros((Bt, h, w, CIN_PAD), dtype=f16, device=dev)
             self.x_g = torch.zeros((Bg, h, w, CIN_PAD), dtype=f16, device=dev)
             self.t_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-            self.coef = torch.zeros(7, dtype=torch.float32, device=dev)
+            self.coef = torch.zeros(8, dtype=torch.float32, device=dev)
+            self.in_scale = torch.ones(1, dtype=torch.float32, device=dev)     # Euler's scale_model_input
+            self.x0_prev = None                                                # DPM-Solver++ state
             self.step_base = torch.zeros(1, dtype=torch.int32, device=dev)   # step index * Bg (hoisted garment K/V)
             self.ctx_t = self.ctx_g = self.aug = None
             self.eps = None
@@ -183,16 +321,30 @@ class TryOnDenoiser:
         self.ctx_g = self.garment.encode_context(text_embeds_cloth.to(dev, f16), out=self.ctx_g)
         self.aug = self.tryon.aug_embedding(add_text_embeds.to(dev, f16), add_time_ids.to(dev), out=self.aug)
 
-    def set_step_tables(self, scheduler, timesteps, garment_keys=None, cache=None):
-        """Uploads the per-step scalars: t and {gs, sqrt(1-abar), 1/sqrt(abar), c0, c1, sigma, phi}, then runs the hoisted
-        garment passes. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments whose
+    def set_step_tables(self, scheduler, timesteps, garment_keys=None, cache=None, eta=0.0):
+        """Uploads the per-step scalars: t (fp32, fractional for Euler's linspace spacing) and the step kernel's
+        coefficients — {gs, sqrt(1-abar), 1/sqrt(abar), c0, c1, sigma, phi} for DDPM, {gs, s, inv_a, p, q, r, sigma_n, k}
+        of b200vton_cfg_solver_step for DDIM (with `eta`), Euler and DPM-Solver++ (solver_step_tables) — then runs the
+        hoisted garment passes. The scheduler kind selects the step's last kernel: switching kinds drops the captured
+        graph. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments whose
         K/V of all steps are cached are copied in instead of recomputed — valid only when the caller guarantees that a
         key identifies (cloth latents, text_embeds_cloth); the timestep list and latent size are added to the key here."""
-        rows = []
-        for t in timesteps:
-            rows.append([self.guidance_scale, *ddpm_step_coefficients(scheduler, int(t)), self.guidance_rescale])
+        kind, coefs, scales, self.step_draws, self.noise_applied = solver_step_tables(scheduler, timesteps, eta)
+        if kind != "ddpm" and self.rescale:
+            raise NotImplementedError("guidance_rescale is implemented for DDPMScheduler only")
+        if kind != getattr(self, "kind", None):
+            self.kind = kind
+            self._graph = None
+        if kind == "dpmpp":
+            if self.x0_prev is None:
+                self.x0_prev = torch.zeros_like(self.latents)
+                self._graph = None
+            self.x0_prev.zero_()
+        rows = [[self.guidance_scale, *c, self.guidance_rescale, 0.0] if kind == "ddpm" else [self.guidance_scale, *c]
+                for c in coefs]
         self.coef_table = torch.tensor(rows, dtype=torch.float32, device=self.device)
-        self.t_table = torch.tensor([float(int(t)) for t in timesteps], dtype=torch.float32, device=self.device)
+        self.scale_table = None if scales is None else torch.tensor(scales, dtype=torch.float32, device=self.device)
+        self.t_table = torch.tensor([float(t) for t in timesteps], dtype=torch.float32, device=self.device)
         T = len(rows)
         self.window = T
         if self.hoist_garment:
@@ -212,7 +364,7 @@ class TryOnDenoiser:
         if self.hoist_garment:
             use_cache = cache is not None and garment_keys is not None and len(garment_keys) == self.Bg and self.window == T
             if use_cache:
-                sig = (tuple(int(t) for t in timesteps), self.h, self.w)
+                sig = (tuple(float(t) for t in timesteps), self.h, self.w)
                 full = [(k, sig) for k in garment_keys]
                 hit = [cache.get(k) for k in full]
                 if all(e is not None for e in hit):
@@ -287,7 +439,10 @@ class TryOnDenoiser:
     def _launch_step(self):
         """The launch sequence of one denoise step over the static buffers (graph-capturable)."""
         L = self.L
-        L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)          # CFG duplication + channel concat as offsets
+        if self.kind == "euler":                                  # scale_model_input on the latent channels only
+            L.nchw_to_nhwc_scaled(self.latents, self.x_t, self.in_scale, c_off=0)
+        else:
+            L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)      # CFG duplication + channel concat as offsets
         temb_t = self.tryon.time_embedding(self.t_dev, self.Bt, self.aug)
         n_persons = self.B if self.do_cfg else 0
         if self.gkv_all is not None:
@@ -298,8 +453,12 @@ class TryOnDenoiser:
             temb_g = self.garment.time_embedding(self.t_dev, self.Bg)
             self.garment.forward(self.x_g, temb_g, self.ctx_g, collect=feats)
             self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=n_persons)
-        step = L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
-        step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
+        if self.kind == "ddpm":
+            step = L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
+            step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
+        else:
+            L.cfg_solver_step(self.eps, self.latents, self.noise if self.kind == "ddim" else None, self.coef, self.kind,
+                              x0_prev=self.x0_prev, do_cfg=self.do_cfg, out=self.latents_next)
         self.latents.copy_(self.latents_next)
 
     # Programmatic dependent launch INSIDE the captured step only (B200VTON_PDL_GRAPH, default below): every kernel node
@@ -314,6 +473,7 @@ class TryOnDenoiser:
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())
         keep = self.latents.clone()
+        keep_x0 = self.x0_prev.clone() if self.kind == "dpmpp" else None     # the warm-up step advances the state
         with torch.cuda.stream(s):
             self._launch_step()
         torch.cuda.current_stream().wait_stream(s)
@@ -329,6 +489,8 @@ class TryOnDenoiser:
             if self.PDL_IN_GRAPH:
                 self.L.set_option("programmatic_launch", pdl_before)
         self.latents.copy_(keep)
+        if keep_x0 is not None:
+            self.x0_prev.copy_(keep_x0)
         self._graph = g
 
     def step(self, i, noise=None, use_graph=True):
@@ -338,6 +500,8 @@ class TryOnDenoiser:
         self.t_dev.copy_(self.t_table[i:i + 1])
         self.coef.copy_(self.coef_table[i])
         self.step_base.copy_(self.base_table[i:i + 1])
+        if self.scale_table is not None:
+            self.in_scale.copy_(self.scale_table[i:i + 1])
         if noise is not None:
             self.noise.copy_(noise)
         else:
@@ -349,6 +513,8 @@ class TryOnDenoiser:
                     self.t_dev.copy_(self.t_table[i:i + 1])
                     self.coef.copy_(self.coef_table[i])
                     self.step_base.copy_(self.base_table[i:i + 1])
+                    if self.scale_table is not None:
+                        self.in_scale.copy_(self.scale_table[i:i + 1])
                 self._graph.replay()
             else:
                 self._launch_step()

@@ -33,6 +33,7 @@ SIGNATURES = {
     "b200vton_groupnorm": [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _f, _i, _vp, _vp, _vp],
     "b200vton_layernorm": [_vp, _i64, _i, _i, _vp, _vp, _f, _vp, _i64, _vp],
     "b200vton_nchw_to_nhwc": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp],
+    "b200vton_nchw_to_nhwc_scaled": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp],
     "b200vton_nhwc_to_nchw": [_vp, _i, _i, _i, _i, _i, _vp, _vp],
     "b200vton_upsample2x_nhwc": [_vp, _i, _i, _i, _i, _vp, _vp],
     "b200vton_im2col3x3_s2_nhwc": [_vp, _i, _i, _i, _i, _vp, _vp],
@@ -40,12 +41,13 @@ SIGNATURES = {
     "b200vton_skinny_linear": [_vp, _i, _i, _i, _vp, _i64, _i, _vp, _i, _i, _vp, _i, _vp, _i, _vp],
     "b200vton_cfg_ddpm_step": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp],
     "b200vton_cfg_rescale_ddpm_step": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp],
+    "b200vton_cfg_solver_step": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp],
     "b200vton_preprocess_inpaint": [_vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "b200vton_postprocess_image": [_vp, _i, _i, _i, _i, _vp, _vp, _vp],
 }
 
 _lib = None
-ABI_VERSION = 107      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
+ABI_VERSION = 108      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
 
 
 def load(build_if_missing=True):
@@ -428,6 +430,18 @@ def nchw_to_nhwc(src, dst, c_off=0):
     return dst
 
 
+def nchw_to_nhwc_scaled(src, dst, scale, c_off=0):
+    """nchw_to_nhwc with dst = fp16(src * scale[0]); scale: one fp32 on the device (a graph replays it per step)."""
+    lib = load()
+    Bs, Cs, H, W = src.shape
+    assert src.is_contiguous() and dst.is_contiguous()
+    assert scale.dtype == torch.float32 and scale.is_cuda and scale.numel() >= 1
+    rc = lib.b200vton_nchw_to_nhwc_scaled(_p(src), Bs, Cs, H, W, _p(dst), dst.shape[0], dst.shape[-1], c_off, _p(scale),
+                                          _stream())
+    _check(rc, "b200vton_nchw_to_nhwc_scaled")
+    return dst
+
+
 def nhwc_to_nchw(src, C, out=None):
     lib = load()
     B, H, W, ldc = src.shape
@@ -543,3 +557,20 @@ def postprocess_image(x, want_pt=True, want_u8=False):
     rc = lib.b200vton_postprocess_image(_p(x), nhwc, B, H, W, _p(pt), _p(u8), _stream())
     _check(rc, "b200vton_postprocess_image")
     return pt, u8
+
+
+SOLVER_KINDS = {"ddim": 0, "euler": 1, "dpmpp": 2}
+
+
+def cfg_solver_step(eps, latents, noise, coef, kind, x0_prev=None, do_cfg=True, out=None):
+    """CFG + one DDIM / Euler / DPM-Solver++ step. eps, latents, noise as cfg_ddpm_step; coef: 8 fp32 on device
+    {gs, s, inv_a, p, q, r, sigma_n, k}; kind: "ddim" | "euler" | "dpmpp"; x0_prev: [B,C,H,W] fp16 state of
+    DPM-Solver++ (read, then overwritten with this step's data prediction)."""
+    lib = load()
+    B, C, H, W = latents.shape
+    if out is None:
+        out = torch.empty_like(latents)
+    rc = lib.b200vton_cfg_solver_step(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(x0_prev), _p(coef),
+                                      SOLVER_KINDS[kind], int(do_cfg), _p(out), _stream())
+    _check(rc, "b200vton_cfg_solver_step")
+    return out

@@ -15,7 +15,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 import torch
 
 from . import clip as _clip
-from .denoise import TryOnDenoiser
+from .denoise import TryOnDenoiser, scheduler_kind
 from .vae import VaeImageProcessor
 
 PipelineImageInput = Any
@@ -325,7 +325,14 @@ class StableDiffusionXLInpaintPipeline:
         return prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds
 
     def prepare_extra_step_kwargs(self, generator, eta):
-        return {"generator": generator}
+        """src/tryon_pipeline.py:746-761: `eta` and `generator` for a scheduler whose `step` takes them."""
+        params = set(inspect.signature(self.scheduler.step).parameters.keys())
+        extra_step_kwargs = {}
+        if "eta" in params:
+            extra_step_kwargs["eta"] = eta
+        if "generator" in params:
+            extra_step_kwargs["generator"] = generator
+        return extra_step_kwargs
 
     def check_inputs(self, prompt, prompt_2, image, mask_image, height, width, strength, callback_steps, output_type,
                      negative_prompt=None, negative_prompt_2=None, prompt_embeds=None, negative_prompt_embeds=None,
@@ -607,6 +614,12 @@ class StableDiffusionXLInpaintPipeline:
         self.check_inputs(prompt, prompt_2, image, mask_image, height, width, strength, callback_steps, output_type,
                           negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
                           callback_on_step_end_tensor_inputs, padding_mask_crop)
+        # the engine's fused step implements DDPM, DDIM, Euler and DPM-Solver++(2M): any other scheduler class raises
+        # here, before any work, instead of being stepped with the wrong update
+        kind = scheduler_kind(self.scheduler)
+        if guidance_rescale > 0 and kind != "ddpm":
+            raise NotImplementedError(f"guidance_rescale with {type(self.scheduler).__name__}: the engine's guidance "
+                                      "rescale is fused with the DDPM step only")
         self._guidance_scale = guidance_scale
         self._guidance_rescale = guidance_rescale
         self._clip_skip = clip_skip
@@ -768,16 +781,22 @@ class StableDiffusionXLInpaintPipeline:
         den.prepare(latents, mask, masked_image_latents, pose_img, cloth, prompt_embeds, add_text_embeds, add_time_ids,
                     image_embeds, text_embeds_cloth.to(device), guidance_scale=self.guidance_scale,
                     do_cfg=self.do_classifier_free_guidance, guidance_rescale=self.guidance_rescale)
-        den.set_step_tables(self.scheduler, timesteps, garment_keys=garment_keys, cache=self.garment_cache)
+        extra_step_kwargs = self.prepare_extra_step_kwargs(generator, eta)
+        den.set_step_tables(self.scheduler, timesteps, garment_keys=garment_keys, cache=self.garment_cache,
+                            eta=extra_step_kwargs.get("eta", 0.0))
         if trace:
             trace.mark("denoiser.prepare (context K/V, garment passes)")
         with self.progress_bar(total=num_inference_steps) as progress_bar:
             for i, t in enumerate(timesteps):
                 if self.interrupt:
                     continue
+                # the variance noise the scheduler's own step would draw, in the same order (DDPM at t > 0, DDIM at
+                # eta > 0, Euler at every step), so the generator ends in the reference's state; Euler's draw is unused
                 step_noise = None
-                if int(t) > 0:                                                               # DDPMScheduler.step
+                if den.step_draws[i]:
                     step_noise = randn_tensor(latents.shape, generator=generator, device=device, dtype=latents.dtype)
+                    if not den.noise_applied:
+                        step_noise = None
                 latents = den.step(i, step_noise, use_graph=self.use_cuda_graph)
                 if callback_on_step_end is not None:
                     callback_kwargs = {k: locals()[k] for k in callback_on_step_end_tensor_inputs}

@@ -150,6 +150,11 @@ int b200vton_layernorm(const void* x, int64_t ldx, int rows, int C, const void* 
  * duplication and the 13-channel concat of src/tryon_pipeline.py:1769,1777 as batch/channel offsets. */
 int b200vton_nchw_to_nhwc(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
                           void* stream);
+/* b200vton_nchw_to_nhwc with dst = fp16(src * scale[0]); scale: one fp32 on device (4-byte aligned, not null). With the
+ * reciprocal 1/sqrt(sigma^2 + 1) it is EulerDiscreteScheduler.scale_model_input on the latent channels
+ * (src/tryon_pipeline.py:1772, before the channel concat of :1777). */
+int b200vton_nchw_to_nhwc_scaled(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
+                                 const void* scale, void* stream);
 /* dst NCHW [B,C,H,W] = src NHWC [B,H,W,ldc][..., :C] */
 int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, void* dst, void* stream);
 
@@ -200,6 +205,16 @@ int b200vton_cfg_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W,
  * b200vton_cfg_ddpm_step (no rescale without CFG, as in the reference). */
 int b200vton_cfg_rescale_ddpm_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
                                    const void* noise, const void* coef, int do_cfg, void* out, void* stream);
+
+/* CFG combine + one step of DDIMScheduler (kind 0), EulerDiscreteScheduler with s_churn = 0 (kind 1) or
+ * DPMSolverMultistepScheduler, dpmsolver++ / midpoint, order 1 or 2 (kind 2); epsilon prediction. Layout of
+ * b200vton_cfg_ddpm_step; coef: 8 fp32 on device {gs, s, inv_a, p, q, r, sigma_n, k}:
+ *   x0 = (x - s g) * inv_a;  D = (1 + k/2) x0 - (k/2) x0_prev;  out = p x + q D + r g + sigma_n noise
+ * with each scheduler's own rounding points (listed at cfg_solver_kernel in elementwise.cu). x0_prev: [B,C,H,W] fp16,
+ * required by kind 2 (read, then overwritten with this step's x0), ignored otherwise. Pointers 2-byte aligned (coef 4). */
+int b200vton_cfg_solver_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                             const void* noise, void* x0_prev, const void* coef, int kind, int do_cfg, void* out,
+                             void* stream);
 
 /* Pre-processing of the inpainting inputs in one launch (diffusers VaeImageProcessor.preprocess for image and mask,
  * the masked image and the latent-resolution mask: src/tryon_pipeline.py:1588-1602, 940-943). image: [B,3,H,W] fp32;
