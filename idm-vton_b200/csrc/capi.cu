@@ -31,7 +31,8 @@ int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* ga
 int nchw_to_nhwc_impl(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
                       const void* scale, cudaStream_t stream);
 int nhwc_to_nchw_impl(const void* src, int B, int C, int H, int W, int ldc, void* dst, cudaStream_t stream);
-int upsample2x_impl(const void* src, int B, int H, int W, int C, void* dst, cudaStream_t stream);
+int upsample_nearest_impl(const void* src, int B, int H, int W, int C, int Hout, int Wout, void* dst,
+                          cudaStream_t stream);
 int im2col_s2_impl(const void* src, int B, int H, int W, int C, void* dst, cudaStream_t stream);
 int timestep_embed_impl(const void* values, int n, int dim, int rows_repeat, void* out, cudaStream_t stream);
 int skinny_linear_impl(const void* x, int ldx, int M, int K, const void* W, long long ldw, int N, const void* bias,
@@ -62,7 +63,7 @@ int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const 
 
 extern "C" {
 
-int b200vton_version(void) { return 108; }
+int b200vton_version(void) { return 109; }
 const char* b200vton_last_error(void) { return vton::get_last_error(); }
 long long b200vton_launch_count(void) { return vton::launch_count(); }
 int b200vton_set_option(const char* name, int value) {
@@ -180,7 +181,11 @@ int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, 
   return vton::nhwc_to_nchw_impl(src, B, C, H, W, ldc, dst, S(stream));
 }
 int b200vton_upsample2x_nhwc(const void* src, int B, int H, int W, int C, void* dst, void* stream) {
-  return vton::upsample2x_impl(src, B, H, W, C, dst, S(stream));
+  return vton::upsample_nearest_impl(src, B, H, W, C, 2 * H, 2 * W, dst, S(stream));
+}
+int b200vton_upsample_nearest_nhwc(const void* src, int B, int H, int W, int C, int Hout, int Wout, void* dst,
+                                   void* stream) {
+  return vton::upsample_nearest_impl(src, B, H, W, C, Hout, Wout, dst, S(stream));
 }
 int b200vton_im2col3x3_s2_nhwc(const void* src, int B, int H, int W, int C, void* dst, void* stream) {
   return vton::im2col_s2_impl(src, B, H, W, C, dst, S(stream));

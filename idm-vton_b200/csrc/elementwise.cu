@@ -65,27 +65,43 @@ int nhwc_to_nchw_impl(const void* src, int B, int C, int H, int W, int ldc, void
 }
 
 // ------------------------------------------------------------------------------------------------
-// Upsample2D data movement: nearest x2 (diffusers Upsample2D = F.interpolate(scale 2, nearest) then conv3x3;
-// built at src/unet_block_hacked_tryon.py:2301,2443). NHWC, 16-byte vectors.
+// Upsample2D data movement: nearest resize to (Hout, Wout) (diffusers Upsample2D = F.interpolate(nearest) then conv3x3;
+// built at src/unet_block_hacked_tryon.py:2301,2443). Scale 2 by default; F.interpolate(size=...) when the UNet forwards
+// an `upsample_size` (latent size not a multiple of 4: src/unet_hacked_tryon.py:1081-1091,1357-1379). NHWC, 16-byte
+// vectors. Source index per axis = ATen's nearest rule (UpSample.h nearest_idx): identity when out == in, dst >> 1 when
+// out == 2 in, else min((int)floorf(dst * scale), in - 1) with scale = (float)in / out.
 // ------------------------------------------------------------------------------------------------
-__global__ void upsample2x_kernel(const uint4* src, int B, int H, int W, int V, uint4* dst) {
+__device__ __forceinline__ int nearest_src(int d, int in, int out, float scale) {
+  if (out == in) return d;
+  if (out == 2 * in) return d >> 1;
+  return min(static_cast<int>(floorf(static_cast<float>(d) * scale)), in - 1);
+}
+
+__global__ void upsample_nearest_kernel(const uint4* src, int B, int H, int W, int V, int Hout, int Wout, float sh,
+                                        float sw, uint4* dst) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long total = static_cast<long long>(B) * 4 * H * W * V;
+  const long long total = static_cast<long long>(B) * Hout * Wout * V;
   if (i >= total) return;
   const int v = static_cast<int>(i % V);
   long long t = i / V;
-  const int x = static_cast<int>(t % (2 * W));
-  t /= 2 * W;
-  const int y = static_cast<int>(t % (2 * H));
-  const int b = static_cast<int>(t / (2 * H));
-  dst[i] = src[((static_cast<long long>(b) * H + (y >> 1)) * W + (x >> 1)) * V + v];
+  const int x = static_cast<int>(t % Wout);
+  t /= Wout;
+  const int y = static_cast<int>(t % Hout);
+  const int b = static_cast<int>(t / Hout);
+  const int sy = nearest_src(y, H, Hout, sh), sx = nearest_src(x, W, Wout, sw);
+  dst[i] = src[((static_cast<long long>(b) * H + sy) * W + sx) * V + v];
 }
 
-int upsample2x_impl(const void* src, int B, int H, int W, int C, void* dst, cudaStream_t stream) {
-  VTON_CHECK_ARG(B > 0 && H > 0 && W > 0 && C % 8 == 0, "upsample2x: bad shape");
-  const long long total = static_cast<long long>(B) * 4 * H * W * (C / 8);
-  upsample2x_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
-      static_cast<const uint4*>(src), B, H, W, C / 8, static_cast<uint4*>(dst));
+int upsample_nearest_impl(const void* src, int B, int H, int W, int C, int Hout, int Wout, void* dst,
+                          cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && Hout > 0 && Wout > 0,
+                 "upsample_nearest: bad shape");
+  VTON_CHECK_ARG(aligned_to(src, 16) && aligned_to(dst, 16), "upsample_nearest: src / dst must be 16-byte aligned");
+  const long long total = static_cast<long long>(B) * Hout * Wout * (C / 8);
+  // scale exactly as ATen computes it for a given output size (compute_scales_value: (float)in / out)
+  const float sh = static_cast<float>(H) / static_cast<float>(Hout), sw = static_cast<float>(W) / static_cast<float>(Wout);
+  upsample_nearest_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+      static_cast<const uint4*>(src), B, H, W, C / 8, Hout, Wout, sh, sw, static_cast<uint4*>(dst));
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;

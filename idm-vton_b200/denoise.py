@@ -204,8 +204,8 @@ def ddpm_step_coefficients(scheduler, t):
 class GarmentKVCache:
     """LRU cache of hoisted garment K/V across requests (SURVEY.md 8f item 4). One entry = the K/V of ONE garment for every
     denoise step and every try-on block ([T, Ng, 2C] fp16 per block: 4.7 GB at 768x1024 / 30 steps), keyed by the caller's
-    garment id plus everything the values depend on (timestep list, latent size). A hit replaces the garment's T
-    garment-UNet passes by device-to-device copies (~2 ms)."""
+    garment id plus everything the values depend on (timestep list, the garment's latent size). A hit replaces the
+    garment's T garment-UNet passes by device-to-device copies (~2 ms)."""
 
     def __init__(self, max_bytes=16 << 30):   # beside 11 GB of weights and the step's K/V on an 80 GB H100
         import collections
@@ -267,8 +267,9 @@ class TryOnDenoiser:
         """guidance_rescale: phi of rescale_noise_cfg (src/tryon_pipeline.py:101-113), applied only under CFG; 0 keeps
         the plain CFG+DDPM kernel. All tensors on the device. latents [B,4,h,w]; mask [Bt,1,h,w], masked_image_latents / pose_latents
         [Bt,4,h,w], prompt_embeds [Bt,77,X], add_text_embeds [Bt,P], add_time_ids [Bt,6], image_embeds [Bt,16,X]
-        with Bt = 2B under CFG ([uncond ; cond] order, src/tryon_pipeline.py:1711-1714); cloth_latents [Bg,4,h,w],
-        text_embeds_cloth [Bg,77,X]."""
+        with Bt = 2B under CFG ([uncond ; cond] order, src/tryon_pipeline.py:1711-1714); cloth_latents [Bg,4,hg,wg],
+        text_embeds_cloth [Bg,77,X]. The garment may have a latent size of its own: the garment UNet runs at the cloth's
+        size (src/tryon_pipeline.py:1654,1787) and its Ng tokens per level join the try-on attention as they are."""
         torch.cuda.nvtx.range_push("b200vton.prepare(context K/V, aug_emb, static input channels)")
         try:
             self._prepare(latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
@@ -282,15 +283,22 @@ class TryOnDenoiser:
         f16 = torch.float16
         B, _, h, w = latents.shape
         Bt = 2 * B if do_cfg else B
-        Bg = cloth_latents.shape[0]
+        Bg, _, hg, wg = cloth_latents.shape
         dev = self.device
+        # the 13-channel concat of src/tryon_pipeline.py:1777 needs every person-side input at the latents' size (the
+        # reference fails in torch.cat otherwise); checked before any buffer is written
+        for name, t in (("mask", mask), ("masked_image_latents", masked_image_latents), ("pose_latents", pose_latents)):
+            if tuple(t.shape[-2:]) != (h, w):
+                raise ValueError(f"{name} has spatial size {tuple(t.shape[-2:])}, the latents {(h, w)}: the try-on UNet "
+                                 "input concatenates them along channels")
         # the rescale flag selects the step's last kernel: a graph captured with the other one must not be replayed
         rescale = bool(do_cfg) and guidance_rescale > 0
-        key = (B, Bt, Bg, h, w, bool(do_cfg), rescale, tuple(prompt_embeds.shape), tuple(image_embeds.shape),
+        key = (B, Bt, Bg, h, w, hg, wg, bool(do_cfg), rescale, tuple(prompt_embeds.shape), tuple(image_embeds.shape),
                tuple(text_embeds_cloth.shape))
         fresh = key != getattr(self, "_key", None)
         self._key = key
         self.B, self.Bt, self.Bg, self.h, self.w = B, Bt, Bg, h, w
+        self.hg, self.wg = hg, wg
         self.do_cfg = do_cfg
         self.guidance_scale = float(guidance_scale)
         self.rescale = rescale
@@ -304,7 +312,7 @@ class TryOnDenoiser:
             self.latents_next = torch.empty_like(self.latents)
             self.noise = torch.zeros_like(self.latents)
             self.x_t = torch.zeros((Bt, h, w, CIN_PAD), dtype=f16, device=dev)
-            self.x_g = torch.zeros((Bg, h, w, CIN_PAD), dtype=f16, device=dev)
+            self.x_g = torch.zeros((Bg, hg, wg, CIN_PAD), dtype=f16, device=dev)   # the garment at its own size
             self.t_dev = torch.zeros(1, dtype=torch.float32, device=dev)
             self.coef = torch.zeros(8, dtype=torch.float32, device=dev)
             self.in_scale = torch.ones(1, dtype=torch.float32, device=dev)     # Euler's scale_model_input
@@ -328,7 +336,8 @@ class TryOnDenoiser:
         hoisted garment passes. The scheduler kind selects the step's last kernel: switching kinds drops the captured
         graph. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments whose
         K/V of all steps are cached are copied in instead of recomputed — valid only when the caller guarantees that a
-        key identifies (cloth latents, text_embeds_cloth); the timestep list and latent size are added to the key here."""
+        key identifies (cloth latents, text_embeds_cloth); the timestep list and the garment's latent size are added to
+        the key here (the person's size does not enter the garment K/V)."""
         kind, coefs, scales, self.step_draws, self.noise_applied = solver_step_tables(scheduler, timesteps, eta)
         if kind != "ddpm" and self.rescale:
             raise NotImplementedError("guidance_rescale is implemented for DDPMScheduler only")
@@ -364,7 +373,7 @@ class TryOnDenoiser:
         if self.hoist_garment:
             use_cache = cache is not None and garment_keys is not None and len(garment_keys) == self.Bg and self.window == T
             if use_cache:
-                sig = (tuple(float(t) for t in timesteps), self.h, self.w)
+                sig = (tuple(float(t) for t in timesteps), self.hg, self.wg)
                 full = [(k, sig) for k in garment_keys]
                 hit = [cache.get(k) for k in full]
                 if all(e is not None for e in hit):
@@ -394,9 +403,10 @@ class TryOnDenoiser:
         return max(1, 64 // max(1, getattr(self, "Bg", 1)))
 
     def kv_bytes_per_step(self):
-        """Bytes of garment K/V one denoise step keeps resident: sum over the try-on blocks of Bg * Ng * 2C fp16."""
+        """Bytes of garment K/V one denoise step keeps resident: sum over the try-on blocks of Bg * Ng * 2C fp16, Ng = the
+        garment's tokens at the block's level (from the cloth latents' size)."""
         ch = self.tryon.ch
-        n, lvl_tokens = (self.h, self.w), {}
+        n, lvl_tokens = (self.hg, self.wg), {}
         for lvl, c in enumerate(ch):
             lvl_tokens[c] = n[0] * n[1]
             n = ((n[0] - 1) // 2 + 1, (n[1] - 1) // 2 + 1)

@@ -373,12 +373,18 @@ class UNetEngine:
         cfg = self.cfg
         n_lvl = len(self.ch)
         state = dict(idx=0, ctx=ctx, gfeats=gfeats, n_persons=n_persons, collect=collect, gkv_pre=gkv_pre)
+        # forward_upsample_size (src/unet_hacked_tryon.py:1081-1091, src/unet_hacked_garmnet.py:994-1000): when this UNet's
+        # own input is not a multiple of 2^num_upsamplers in either dimension, every upsampler resizes to the size of the
+        # next skip it will be concatenated with instead of doubling (the stride-2 convolutions round up)
         div = 2 ** (n_lvl - 1)
-        if x_in.shape[1] % div or x_in.shape[2] % div:
-            # diffusers pads the up path with `upsample_size` when the latent size is not a multiple of the total
-            # downsampling factor (src/unet_hacked_tryon.py:1051-1064); inference.py never gets there (768x1024 -> 128x96)
-            raise NotImplementedError(f"latent size {tuple(x_in.shape[1:3])} must be a multiple of {div} (pixel size a "
-                                      f"multiple of {8 * div}): the reference's `upsample_size` path is not implemented")
+        forward_upsample_size = x_in.shape[1] % div != 0 or x_in.shape[2] % div != 0
+        if forward_upsample_size and getattr(L, "upsample_nearest", None) is None:
+            # the resize to a skip's size is a kernel of its own (b200vton_upsample_nearest_nhwc): a binding without it
+            # cannot run this size, and says so before the first launch instead of failing deep inside the up path
+            raise NotImplementedError(f"latent size {tuple(x_in.shape[1:3])} is not a multiple of {div} (pixel size a "
+                                      f"multiple of {8 * div}): the reference's `upsample_size` path needs the "
+                                      "nearest-resize kernel b200vton_upsample_nearest_nhwc, which this library binding "
+                                      "does not provide")
         x = L.conv3x3(x_in, self.w_in, bias=self.b_in)
         skips = [x]
         for i, lvl in enumerate(self.down):
@@ -400,7 +406,9 @@ class UNetEngine:
                 if lvl["attn"]:
                     x = self._t2d(lvl["attn"][j], x, state)
             if lvl["up"] is not None:
-                x = L.conv3x3(L.upsample2x(x), lvl["up"][0], bias=lvl["up"][1])
+                # (the reference's upsample_size = down_block_res_samples[-1].shape[2:] after this block's pops, :1357-1362)
+                up = L.upsample_nearest(x, skips[-1].shape[1:3]) if forward_upsample_size else L.upsample2x(x)
+                x = L.conv3x3(up, lvl["up"][0], bias=lvl["up"][1])
         if self.kind != "tryon":
             return None
         h = L.groupnorm(x, self.no_w, self.no_b, 1e-5, True)

@@ -36,6 +36,7 @@ SIGNATURES = {
     "b200vton_nchw_to_nhwc_scaled": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp],
     "b200vton_nhwc_to_nchw": [_vp, _i, _i, _i, _i, _i, _vp, _vp],
     "b200vton_upsample2x_nhwc": [_vp, _i, _i, _i, _i, _vp, _vp],
+    "b200vton_upsample_nearest_nhwc": [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp],
     "b200vton_im2col3x3_s2_nhwc": [_vp, _i, _i, _i, _i, _vp, _vp],
     "b200vton_timestep_embedding": [_vp, _i, _i, _i, _vp, _vp],
     "b200vton_skinny_linear": [_vp, _i, _i, _i, _vp, _i64, _i, _vp, _i, _i, _vp, _i, _vp, _i, _vp],
@@ -47,7 +48,7 @@ SIGNATURES = {
 }
 
 _lib = None
-ABI_VERSION = 108      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
+ABI_VERSION = 109      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
 
 
 def load(build_if_missing=True):
@@ -420,11 +421,26 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     return out
 
 
+def _check_scatter_shapes(src, dst, c_off):
+    """The C ABI takes H, W from the source only: a dst of another size would be written out of bounds (larger src) or
+    left partly unwritten (smaller src), so the sizes are compared here, before any launch."""
+    if src.dim() != 4 or dst.dim() != 4:
+        raise ValueError(f"nchw_to_nhwc: src must be [B,C,H,W] and dst [B,H,W,ldc], got {tuple(src.shape)} and "
+                         f"{tuple(dst.shape)}")
+    if tuple(src.shape[2:]) != tuple(dst.shape[1:3]):
+        raise ValueError(f"nchw_to_nhwc: src spatial size {tuple(src.shape[2:])} differs from dst's "
+                         f"{tuple(dst.shape[1:3])}")
+    if c_off < 0 or c_off + src.shape[1] > dst.shape[3]:
+        raise ValueError(f"nchw_to_nhwc: channels [{c_off}, {c_off + src.shape[1]}) do not fit dst's {dst.shape[3]}")
+    if not (src.is_contiguous() and dst.is_contiguous()):
+        raise ValueError("nchw_to_nhwc: src and dst must be contiguous")
+
+
 def nchw_to_nhwc(src, dst, c_off=0):
-    """dst[s,y,x,c_off+c] = src[s % Bs, c, y, x]; dst: [Bd,H,W,ldc] contiguous."""
+    """dst[s,y,x,c_off+c] = src[s % Bs, c, y, x]; dst: [Bd,H,W,ldc] contiguous, the same H, W as src."""
+    _check_scatter_shapes(src, dst, c_off)
     lib = load()
     Bs, Cs, H, W = src.shape
-    assert src.is_contiguous() and dst.is_contiguous()
     rc = lib.b200vton_nchw_to_nhwc(_p(src), Bs, Cs, H, W, _p(dst), dst.shape[0], dst.shape[-1], c_off, _stream())
     _check(rc, "b200vton_nchw_to_nhwc")
     return dst
@@ -432,9 +448,9 @@ def nchw_to_nhwc(src, dst, c_off=0):
 
 def nchw_to_nhwc_scaled(src, dst, scale, c_off=0):
     """nchw_to_nhwc with dst = fp16(src * scale[0]); scale: one fp32 on the device (a graph replays it per step)."""
+    _check_scatter_shapes(src, dst, c_off)
     lib = load()
     Bs, Cs, H, W = src.shape
-    assert src.is_contiguous() and dst.is_contiguous()
     assert scale.dtype == torch.float32 and scale.is_cuda and scale.numel() >= 1
     rc = lib.b200vton_nchw_to_nhwc_scaled(_p(src), Bs, Cs, H, W, _p(dst), dst.shape[0], dst.shape[-1], c_off, _p(scale),
                                           _stream())
@@ -459,6 +475,21 @@ def upsample2x(x, out=None):
         out = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float16, device=x.device)
     rc = lib.b200vton_upsample2x_nhwc(_p(x), B, H, W, C, _p(out), _stream())
     _check(rc, "b200vton_upsample2x_nhwc")
+    return out
+
+
+def upsample_nearest(x, size, out=None):
+    """x: [B,H,W,C] NHWC fp16 (contiguous) -> [B,Hout,Wout,C], F.interpolate(size=(Hout, Wout), mode="nearest")."""
+    lib = load()
+    _f16(x, "x")
+    B, H, W, C = x.shape
+    Hout, Wout = int(size[0]), int(size[1])
+    assert x.is_contiguous()
+    if out is None:
+        out = torch.empty((B, Hout, Wout, C), dtype=torch.float16, device=x.device)
+    assert out.shape == (B, Hout, Wout, C) and out.is_contiguous()
+    rc = lib.b200vton_upsample_nearest_nhwc(_p(x), B, H, W, C, Hout, Wout, _p(out), _stream())
+    _check(rc, "b200vton_upsample_nearest_nhwc")
     return out
 
 

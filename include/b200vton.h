@@ -158,8 +158,15 @@ int b200vton_nchw_to_nhwc_scaled(const void* src, int Bs, int Cs, int H, int W, 
 /* dst NCHW [B,C,H,W] = src NHWC [B,H,W,ldc][..., :C] */
 int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, void* dst, void* stream);
 
-/* nearest-neighbour x2 (diffusers Upsample2D's F.interpolate), NHWC */
+/* nearest-neighbour x2 (diffusers Upsample2D's F.interpolate), NHWC; = b200vton_upsample_nearest_nhwc to (2H, 2W) */
 int b200vton_upsample2x_nhwc(const void* src, int B, int H, int W, int C, void* dst, void* stream);
+/* nearest-neighbour resize src [B,H,W,C] -> dst [B,Hout,Wout,C], NHWC, C % 8 == 0, src / dst 16-byte aligned: diffusers
+ * Upsample2D's F.interpolate(size=upsample_size, mode="nearest") when the UNet forwards an upsample size (latent size not a
+ * multiple of 2^num_upsamplers: src/unet_hacked_tryon.py:1081-1091,1357-1379, src/unet_hacked_garmnet.py:994-1000,
+ * 1264-1274). Source index per axis as ATen's `nearest` mode: identity when out == in, dst >> 1 when out == 2 in,
+ * otherwise min((int)floorf(dst * ((float)in / out)), in - 1). */
+int b200vton_upsample_nearest_nhwc(const void* src, int B, int H, int W, int C, int Hout, int Wout, void* dst,
+                                   void* stream);
 /* patches of a 3x3 stride-2 pad-1 conv (diffusers Downsample2D) as A[B*Ho*Wo, 9*C], K ordered tap-major */
 int b200vton_im2col3x3_s2_nhwc(const void* src, int B, int H, int W, int C, void* dst, void* stream);
 
