@@ -252,10 +252,12 @@ def token_embedding(ids, tok, pos, T):
     return out
 
 
-def conv3x3_f32_supported(x, cin, cout):
-    """Shapes the TF32 convolution kernel covers (everything else stays on the caller's fallback)."""
+def conv3x3_f32_supported(x, cin, cout, width=None):
+    """Shapes the TF32 convolution kernel covers (everything else stays on the caller's fallback). width: the width of
+    the convolution's input when it is not x's own (x taken before a 2x upsampling)."""
+    w = x.shape[3] if width is None else width
     return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and cin % 32 == 0 and cout % 32 == 0 and cout >= 64
-            and x.shape[3] % 8 == 0)
+            and w % 8 == 0)
 
 
 def pack_conv3x3_f32(weight):

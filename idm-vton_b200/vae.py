@@ -57,29 +57,45 @@ _ENGINE_FUSED = os.environ.get("B200VTON_VAE_FUSED", "1") == "1"                
 _ATTN_FUSED = os.environ.get("B200VTON_VAE_ATTN_FUSED", "1") == "1"           # one-pass split / softmax-split kernels
 
 
-def _conv(conv, x, residual=None):
-    """3x3 / stride 1 / pad 1 fp32 convolutions with 32-aligned channel counts run on the engine's TF32 tensor-core
-    kernel on CUDA (`b200vton_conv3x3_nhwc_f32`: TF32 products, fp32 accumulation — the arithmetic class cuDNN uses for
-    fp32 convolutions under torch's default `allow_tf32`); every other case (CPU, fp16, conv_in / conv_out with 3-8
-    channels, stride-2 downsamplers, 1x1 shortcuts, TF32 disabled by the caller) stays on `nn.Conv2d`."""
+def _tf32_engine(conv, x, width=None):
+    """True when `_conv(conv, x)` runs on the engine's TF32 convolution; width: its input's width when x is taken before
+    the 2x upsampling that produces that input."""
     if (_conv_device_ok(x) and x.dtype == torch.float32 and conv.kernel_size == (3, 3) and conv.stride == (1, 1)
             and conv.padding == (1, 1) and conv.dilation == (1, 1) and conv.groups == 1
             and torch.backends.cudnn.allow_tf32 and (_ENGINE_CONV or _ENGINE_NHWC)):
         from . import lib as L
-        if L.conv3x3_f32_supported(x, conv.in_channels, conv.out_channels):
-            key = (conv.weight.data_ptr(), conv.weight._version)
-            cache = getattr(conv, "_b200_packed", None)
-            if cache is None or cache[0] != key:
-                cache = (key, L.pack_conv3x3_f32(conv.weight))
-                conv._b200_packed = cache
-            if residual is not None and not _ENGINE_FUSED:
-                return residual + L.conv3x3_f32(x, cache[1], conv.bias)
-            return L.conv3x3_f32(x, cache[1], conv.bias, residual=residual)
+        if width is None:
+            return L.conv3x3_f32_supported(x, conv.in_channels, conv.out_channels)
+        return L.conv3x3_f32_supported(x, conv.in_channels, conv.out_channels, width=width)
+    return False
+
+
+def _conv(conv, x, residual=None):
+    """3x3 / stride 1 / pad 1 fp32 convolutions with 32-aligned channel counts run on the engine's TF32 tensor-core
+    kernel on CUDA (`b200vton_conv3x3_nhwc_f32`: TF32 products, fp32 accumulation — the arithmetic class cuDNN uses for
+    fp32 convolutions under torch's default `allow_tf32`); every other case (CPU, fp16, conv_in / conv_out with 3-8
+    channels, stride-2 downsamplers, 1x1 shortcuts, TF32 disabled by the caller) stays on `nn.Conv2d`.
+    The tensor core truncates its fp32 operands (it ignores their 13 low mantissa bits) where cuDNN rounds them to
+    nearest; truncation shrinks every product, a slope of 1 - 7e-4 against the exact convolution (measured on an H100,
+    tests/test_vae_parity_gpu.py). So on the device the packed weights are rounded to nearest once, and `_Up` rounds the
+    input (the only caller whose input is not already fp16 from the norm)."""
+    if _tf32_engine(conv, x):
+        from . import lib as L
+        key = (conv.weight.data_ptr(), conv.weight._version)
+        cache = getattr(conv, "_b200_packed", None)
+        if cache is None or cache[0] != key:
+            w = L.pack_conv3x3_f32(conv.weight)
+            cache = (key, _tf32(w) if w.is_cuda else w)     # only the tensor core truncates: nothing to compensate on a CPU
+            conv._b200_packed = cache
+        if residual is not None and not _ENGINE_FUSED:
+            return residual + L.conv3x3_f32(x, cache[1], conv.bias)
+        return L.conv3x3_f32(x, cache[1], conv.bias, residual=residual)
     return conv(x) if residual is None else residual + conv(x)
 
 
-# GroupNorm(+SiLU) -> convolution with an fp16 hand-off: the TF32 convolution rounds its fp32 operands to 10 mantissa bits
-# anyway, so the norm stores fp16 (same mantissa; its outputs are O(1-10), far inside fp16's range) and the convolution runs
+# GroupNorm(+SiLU) -> convolution with an fp16 hand-off: the TF32 convolution reduces its fp32 operands to 10 mantissa bits
+# anyway, so the norm stores fp16 (same mantissa, rounded to nearest as cuDNN's TF32 convolutions round; its outputs are
+# O(1-10), far inside fp16's range) and the convolution runs
 # with fp16 operands — half the norm's write and the convolution's read, twice the MMA rate, fp32 accumulation / bias /
 # residual / output as before (`b200vton_conv3x3_nhwc_f16in_f32`). B200VTON_VAE_F16ACT=0 keeps the fp32 hand-off.
 _F16_ACT = os.environ.get("B200VTON_VAE_F16ACT", "1") == "1"
@@ -119,14 +135,24 @@ class _Resnet(nn.Module):
         return _gn_silu_conv(self.norm2, self.conv2, h, residual=x)        # x + conv2(silu(norm2(h)))
 
 
+def _tf32(t):
+    """fp32 -> the nearest TF32 value (10 mantissa bits, ties away from zero), still fp32: round half up on the 13 low
+    mantissa bits, then clear them."""
+    return ((t.view(torch.int32) + 4096) & -8192).view(torch.float32)
+
+
+def _tf32_(t):
+    """`_tf32` in place (no temporaries: the decoder's largest upsampler input is 200 MB)."""
+    t.view(torch.int32).add_(4096).bitwise_and_(-8192)
+    return t
+
+
 def _split_tf32(x):
     """x ~ hi + lo with BOTH parts exactly representable in TF32 (10 mantissa bits): hi = tf32(x), lo = tf32(x - hi), so the
-    tensor core — which ignores the 13 low mantissa bits of its fp32 operands, i.e. truncates — sees them unchanged
+    tensor core — which ignores the 13 low mantissa bits of its fp32 operands, i.e. truncates — sees them unchanged.
     What is dropped is 2^-22 |x|."""
-    def tf32(t):
-        return ((t.view(torch.int32) + 4096) & -8192).view(torch.float32)   # round half up on the 13 low bits, clear them
-    hi = tf32(x)
-    return hi, tf32(x - hi)
+    hi = _tf32(x)
+    return hi, _tf32(x - hi)
 
 
 def _attention_fp32_3xtf32(q, k, v, chunk=2048):
@@ -135,9 +161,9 @@ def _attention_fp32_3xtf32(q, k, v, chunk=2048):
     memory-efficient kernel uses no tensor cores. Here every product runs on the TF32
     tensor cores three times with split operands — a·b ≈ a_hi·b_hi + a_hi·b_lo + a_lo·b_hi, fp32 accumulation — which
     removes the TF32 operand rounding (the dropped a_lo·b_lo term is 2^-22 relative); what remains is the tensor core's own
-    fp32 accumulation over thousands of keys: 3.9e-5 max abs error against fp64 at 3072 keys where fp32 SDPA has 3.6e-6
-    and a single TF32 pass 3.0e-3 (tests/test_kernels_gpu.py) — an order below the error of the TF32 convolutions around
-    it. Queries are processed in chunks so the score block stays small. The products are cuBLAS TF32 GEMMs; the split operands and
+    fp32 accumulation over thousands of keys, which grows with their number: 5e-6 to 5e-5 of the output scale against
+    fp64 at 1155 to 12 288 keys, where fp32 SDPA has 1-2e-6 and a single TF32 pass 5-8e-4 (H100,
+    tests/test_vae_parity_gpu.py) — an order below the error of the TF32 convolutions around it. Queries are processed in chunks so the score block stays small. The products are cuBLAS TF32 GEMMs; the split operands and
     the softmax come from `b200vton_split_tf32` / `b200vton_softmax_split_tf32` (one pass each; the three score products are ONE
     GEMM over the concatenated contraction [q_lo | q_hi | q_hi] . [k_hi | k_lo | k_hi]^T, small terms first); `_ATTN_FUSED = False` is the ATen formulation
     of the same arithmetic (kept as the cross-check of tests/test_kernels_gpu.py). Host-side plumbing of a SURVEY 8f row."""
@@ -246,7 +272,12 @@ class _Up(nn.Module):
         for r in self.resnets:
             x = r(x)
         if self.upsamplers is not None:
-            x = _conv(self.upsamplers[0].conv, F.interpolate(x, scale_factor=2.0, mode="nearest"))
+            conv = self.upsamplers[0].conv
+            # the engine's TF32 convolution truncates its input: round it to nearest first, before the upsampling, where
+            # it is a quarter of the size (nearest upsampling copies values, so the rounding commutes with it)
+            if x.is_cuda and _tf32_engine(conv, x, width=2 * x.shape[3]):
+                x = _tf32_(x)                      # in place: x is the last resnet's fresh output, read by nothing else
+            x = _conv(conv, F.interpolate(x, scale_factor=2.0, mode="nearest"))
         return x
 
 
