@@ -29,7 +29,7 @@ int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW
 int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
                    void* out, long long ldo, cudaStream_t stream);
 int nchw_to_nhwc_impl(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
-                      const void* scale, cudaStream_t stream);
+                      const void* scale, cudaStream_t stream, bool scale_rows = false);
 int nhwc_to_nchw_impl(const void* src, int B, int C, int H, int W, int ldc, void* dst, cudaStream_t stream);
 int upsample_nearest_impl(const void* src, int B, int H, int W, int C, int Hout, int Wout, void* dst,
                           cudaStream_t stream);
@@ -57,6 +57,11 @@ int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, 
                           const void* coef, int do_cfg, void* out, cudaStream_t stream);
 int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
                     void* x0_prev, const void* coef, int kind, int do_cfg, void* out, cudaStream_t stream);
+int cfg_ddpm_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                       const void* coef, int coef_stride, int do_cfg, void* out, cudaStream_t stream);
+int cfg_solver_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                         void* x0_prev, const void* coef, int coef_stride, int kind, int do_cfg, void* out,
+                         cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
@@ -177,6 +182,13 @@ int b200vton_nchw_to_nhwc_scaled(const void* src, int Bs, int Cs, int H, int W, 
   VTON_CHECK_ARG(scale, "nchw_to_nhwc_scaled: scale is null");
   return vton::nchw_to_nhwc_impl(src, Bs, Cs, H, W, dst, Bd, ldc, c_off, scale, S(stream));
 }
+int b200vton_nchw_to_nhwc_scaled_rows(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc,
+                                      int c_off, const void* scale, void* stream) {
+  VTON_CHECK_ARG(src && dst && scale, "nchw_to_nhwc_scaled_rows: null pointer");
+  VTON_CHECK_ARG(vton::aligned_to(src, 2) && vton::aligned_to(dst, 2),
+                 "nchw_to_nhwc_scaled_rows: src and dst must be 2-byte aligned");
+  return vton::nchw_to_nhwc_impl(src, Bs, Cs, H, W, dst, Bd, ldc, c_off, scale, S(stream), true);
+}
 int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, void* dst, void* stream) {
   return vton::nhwc_to_nchw_impl(src, B, C, H, W, ldc, dst, S(stream));
 }
@@ -211,6 +223,17 @@ int b200vton_cfg_solver_step(const void* eps, int ldc, int B, int C, int H, int 
                              const void* noise, void* x0_prev, const void* coef, int kind, int do_cfg, void* out,
                              void* stream) {
   return vton::cfg_solver_impl(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, kind, do_cfg, out, S(stream));
+}
+int b200vton_cfg_ddpm_step_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                const void* noise, const void* coef, int coef_stride, int do_cfg, void* out,
+                                void* stream) {
+  return vton::cfg_ddpm_rows_impl(eps, ldc, B, C, H, W, latents, noise, coef, coef_stride, do_cfg, out, S(stream));
+}
+int b200vton_cfg_solver_step_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                  const void* noise, void* x0_prev, const void* coef, int coef_stride, int kind,
+                                  int do_cfg, void* out, void* stream) {
+  return vton::cfg_solver_rows_impl(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, coef_stride, kind, do_cfg, out,
+                                    S(stream));
 }
 
 int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_channels, const void* image_min, int B,

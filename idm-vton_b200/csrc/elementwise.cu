@@ -14,6 +14,9 @@ namespace vton {
 // scale (device scalar, may be null): dst = fp16(src * scale[0]) instead of a copy. This is the
 // `scheduler.scale_model_input` of EulerDiscreteScheduler (src/tryon_pipeline.py:1772): the caller passes the fp32
 // reciprocal 1 / sqrt(sigma^2 + 1), because torch divides a CUDA tensor by a CPU scalar as a product with its reciprocal.
+// ROWS (the `_rows` entry point): scale holds one fp32 per source sample and dst row s is scaled by scale[s % Bs], so the
+// CFG duplicate rows b and b + Bs share sample b's scale (per-slot step indices of the continuous-batching denoiser).
+template <bool ROWS>
 __global__ void nchw_to_nhwc_kernel(const __half* src, int Bs, int Cs, int HW, __half* dst, int Bd, int ldc, int c_off,
                                     const float* scale) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -23,7 +26,7 @@ __global__ void nchw_to_nhwc_kernel(const __half* src, int Bs, int Cs, int HW, _
   const int px = static_cast<int>(i % HW);
   const int sb = s % Bs;
   if (scale) {
-    const float f = *scale;
+    const float f = ROWS ? scale[sb] : *scale;
     for (int c = 0; c < Cs; ++c)
       dst[i * ldc + c_off + c] = f2h(h2f(src[(static_cast<long long>(sb) * Cs + c) * HW + px]) * f);
   } else {
@@ -42,11 +45,12 @@ __global__ void nhwc_to_nchw_kernel(const __half* src, int B, int C, int HW, int
 }
 
 int nchw_to_nhwc_impl(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
-                      const void* scale, cudaStream_t stream) {
+                      const void* scale, cudaStream_t stream, bool scale_rows) {
   VTON_CHECK_ARG(Bs > 0 && Cs > 0 && H > 0 && W > 0 && Bd > 0 && c_off + Cs <= ldc, "nchw_to_nhwc: bad shape");
   VTON_CHECK_ARG(aligned_to(scale, 4), "nchw_to_nhwc: scale must be 4-byte aligned");
   const long long total = static_cast<long long>(Bd) * H * W;
-  nchw_to_nhwc_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+  auto kern = scale_rows ? nchw_to_nhwc_kernel<true> : nchw_to_nhwc_kernel<false>;
+  kern<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
       static_cast<const __half*>(src), Bs, Cs, H * W, static_cast<__half*>(dst), Bd, ldc, c_off,
       static_cast<const float*>(scale));
   count_launch();
@@ -260,15 +264,19 @@ int skinny_linear_impl(const void* x, int ldx, int M, int K, const void* W, long
 //   prev = fp16(fp16(c0 * x0) + fp16(c1 * x));  out = prev + fp16(sigma * noise)   (noise == null at t == 0)
 // eps: NHWC [2B, HW, ldc] (uncond rows first, then cond); latents/noise/out: NCHW [B, 4, HW]. Coefficients live on the
 // device ([6] floats: gs, sb, inv_sa, c0, c1, sigma) so a captured CUDA graph can be replayed for every step.
+// ROWS (b200vton_cfg_ddpm_step_rows): coef is [B, coef_stride] and sample b reads row b, so every sample of the batch
+// can be at its own denoise step (continuous batching); coef_stride 0 is the single-row kernel.
 // ------------------------------------------------------------------------------------------------
+template <bool ROWS>
 __global__ void cfg_ddpm_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents,
-                                const __half* noise, const float* coef, int do_cfg, __half* out) {
+                                const __half* noise, const float* coef, int coef_stride, int do_cfg, __half* out) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(B) * C * HW;
   if (i >= total) return;
   const int px = static_cast<int>(i % HW);
   const int c = static_cast<int>((i / HW) % C);
   const int b = static_cast<int>(i / (static_cast<long long>(HW) * C));
+  if (ROWS) coef += static_cast<long long>(b) * coef_stride;
   const float gs = coef[0], sb = coef[1], inv_sa = coef[2], c0 = coef[3], c1 = coef[4], sigma = coef[5];
   float g;
   if (do_cfg) {
@@ -285,16 +293,38 @@ __global__ void cfg_ddpm_kernel(const __half* eps, int ldc, int B, int C, int HW
   out[i] = f2h(prev);
 }
 
-int cfg_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
-                  const void* coef, int do_cfg, void* out, cudaStream_t stream) {
-  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef, "cfg_ddpm: bad arguments");
+template <bool ROWS>
+static int launch_cfg_ddpm(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                           const void* coef, int coef_stride, int do_cfg, void* out, cudaStream_t stream) {
   const long long total = static_cast<long long>(B) * C * H * W;
-  cfg_ddpm_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+  cfg_ddpm_kernel<ROWS><<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
       static_cast<const __half*>(eps), ldc, B, C, H * W, static_cast<const __half*>(latents),
-      static_cast<const __half*>(noise), static_cast<const float*>(coef), do_cfg, static_cast<__half*>(out));
+      static_cast<const __half*>(noise), static_cast<const float*>(coef), coef_stride, do_cfg,
+      static_cast<__half*>(out));
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;
+}
+
+int cfg_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                  const void* coef, int do_cfg, void* out, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef, "cfg_ddpm: bad arguments");
+  return launch_cfg_ddpm<false>(eps, ldc, B, C, H, W, latents, noise, coef, 0, do_cfg, out, stream);
+}
+
+constexpr int kDdpmCoefs = 6;      // {gs, sb, inv_sa, c0, c1, sigma}
+constexpr int kSolverCoefs = 8;    // {gs, s, inv_a, p, q, r, sigma_n, k}
+
+int cfg_ddpm_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                       const void* coef, int coef_stride, int do_cfg, void* out, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef && eps && latents && out,
+                 "cfg_ddpm_rows: bad arguments");
+  VTON_CHECK_ARG(coef_stride == 0 || coef_stride >= kDdpmCoefs,
+                 "cfg_ddpm_rows: coef_stride %d is neither 0 nor >= %d", coef_stride, kDdpmCoefs);
+  VTON_CHECK_ARG(aligned_to(eps, 2) && aligned_to(latents, 2) && aligned_to(noise, 2) && aligned_to(out, 2) &&
+                     aligned_to(coef, 4),
+                 "cfg_ddpm_rows: fp16 operands must be 2-byte aligned and coef 4-byte aligned");
+  return launch_cfg_ddpm<true>(eps, ldc, B, C, H, W, latents, noise, coef, coef_stride, do_cfg, out, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -414,15 +444,18 @@ int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, 
 //          out = fp16((p x + fp16(q x0)) + fp16(fp32(q / 2) * fp16(k * fp16(x0 - x0_prev))));  x0_prev = x0
 // sigma_n * noise is added the same way by every kind when noise is not null (only DDIM with eta > 0 draws it).
 // ------------------------------------------------------------------------------------------------
-template <int KIND>
+// ROWS (b200vton_cfg_solver_step_rows): coef is [B, coef_stride], sample b reads row b (coef_stride 0: one row for all).
+template <int KIND, bool ROWS>
 __global__ void cfg_solver_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents,
-                                  const __half* noise, __half* x0_prev, const float* coef, int do_cfg, __half* out) {
+                                  const __half* noise, __half* x0_prev, const float* coef, int coef_stride, int do_cfg,
+                                  __half* out) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long total = static_cast<long long>(B) * C * HW;
   if (i >= total) return;
   const int px = static_cast<int>(i % HW);
   const int c = static_cast<int>((i / HW) % C);
   const int b = static_cast<int>(i / (static_cast<long long>(HW) * C));
+  if (ROWS) coef += static_cast<long long>(b) * coef_stride;
   const float gs = coef[0], s = coef[1], inv_a = coef[2], p = coef[3], q = coef[4], r = coef[5], sigma_n = coef[6],
               k = coef[7];
   float g;
@@ -452,12 +485,16 @@ __global__ void cfg_solver_kernel(const __half* eps, int ldc, int B, int C, int 
   out[i] = f2h(prev);
 }
 
-int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
-                    void* x0_prev, const void* coef, int kind, int do_cfg, void* out, cudaStream_t stream) {
+template <bool ROWS>
+static int launch_cfg_solver(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                             const void* noise, void* x0_prev, const void* coef, int coef_stride, int kind, int do_cfg,
+                             void* out, cudaStream_t stream) {
   VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && coef && eps && latents && out,
                  "cfg_solver: bad arguments");
   VTON_CHECK_ARG(kind >= 0 && kind <= 2, "cfg_solver: kind %d is not 0 (DDIM), 1 (Euler) or 2 (DPM-Solver++)", kind);
   VTON_CHECK_ARG(kind != 2 || x0_prev, "cfg_solver: DPM-Solver++ needs the x0_prev state buffer");
+  VTON_CHECK_ARG(coef_stride == 0 || coef_stride >= kSolverCoefs,
+                 "cfg_solver: coef_stride %d is neither 0 nor >= %d", coef_stride, kSolverCoefs);
   VTON_CHECK_ARG(aligned_to(eps, 2) && aligned_to(latents, 2) && aligned_to(noise, 2) && aligned_to(x0_prev, 2) &&
                      aligned_to(out, 2) && aligned_to(coef, 4),
                  "cfg_solver: fp16 operands must be 2-byte aligned and coef 4-byte aligned");
@@ -470,14 +507,26 @@ int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const 
   auto cf = static_cast<const float*>(coef);
   auto o = static_cast<__half*>(out);
   if (kind == 0)
-    cfg_solver_kernel<0><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, do_cfg, o);
+    cfg_solver_kernel<0, ROWS><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, coef_stride, do_cfg, o);
   else if (kind == 1)
-    cfg_solver_kernel<1><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, do_cfg, o);
+    cfg_solver_kernel<1, ROWS><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, nullptr, cf, coef_stride, do_cfg, o);
   else
-    cfg_solver_kernel<2><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, x0p, cf, do_cfg, o);
+    cfg_solver_kernel<2, ROWS><<<grid, 256, 0, stream>>>(e, ldc, B, C, H * W, l, n, x0p, cf, coef_stride, do_cfg, o);
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;
+}
+
+int cfg_solver_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                    void* x0_prev, const void* coef, int kind, int do_cfg, void* out, cudaStream_t stream) {
+  return launch_cfg_solver<false>(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, 0, kind, do_cfg, out, stream);
+}
+
+int cfg_solver_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                         void* x0_prev, const void* coef, int coef_stride, int kind, int do_cfg, void* out,
+                         cudaStream_t stream) {
+  return launch_cfg_solver<true>(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, coef_stride, kind, do_cfg, out,
+                                 stream);
 }
 
 // ------------------------------------------------------------------------------------------------

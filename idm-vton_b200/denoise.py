@@ -529,3 +529,183 @@ class TryOnDenoiser:
             else:
                 self._launch_step()
         return self.latents
+
+
+def identity_step_row(kind):
+    """The coefficient row of an idle slot of SlotDenoiser: the step returns its latents unchanged (zeros stay zeros),
+    whatever the finite eps. DDPM {gs, sb, inv_sa, c0, c1, sigma, phi, 0}: x0 = 0, prev = 1 * x; DDIM and DPM-Solver++
+    {gs, s, inv_a, p, q, r, sigma_n, k}: x0 = x, out = fp16(1 * x0) (DDIM) or 1 * x + fp16(0 * x0) (DPM++); Euler:
+    x0 = x - 0, d = 0, out = x + 0."""
+    return {"ddpm": [0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0],
+            "ddim": [0.0, 0.0, 1.0, 0.0, 1.0, 0.0, 0.0, 0.0],
+            "euler": [0.0] * 8,
+            "dpmpp": [0.0, 0.0, 1.0, 1.0, 0.0, 0.0, 0.0, 0.0]}[kind]
+
+
+class SlotDenoiser:
+    """The denoise step of continuous batching: S slots, each holding one request at its own step index.
+
+    Every buffer is indexed by slot: [S, ...] for persons and garments, [2S, ...] for the try-on batch under CFG (uncond
+    row s, cond row S + s). One step is one CUDA graph per capacity: the latent scatter, the garment UNet at batch S with
+    per-slot timesteps, the try-on UNet at batch 2S with the garment features of slot s streamed into rows s / S + s, and
+    the step kernel that reads one coefficient row per slot (b200vton_cfg_*_step_rows). Before each replay the host
+    gathers each slot's timestep / coefficient / input-scale row from the per-step tables into the static buffers, with
+    copies issued outside the graph (with B200VTON_PDL_GRAPH every kernel node of the graph is a library kernel).
+
+    The garment passes stay in the step: slots at different phases cannot share K/V hoisted over all steps of one request
+    (kv_bytes_per_step x T per garment), so GarmentKVCache does not apply here. Idle slots hold zeros and the identity
+    coefficient row (identity_step_row); their outputs are ignored. No row of one slot enters another slot's result, so at
+    a fixed S a request's result does not depend on which slot it runs in or on what the other slots hold."""
+
+    PDL_IN_GRAPH = TryOnDenoiser.PDL_IN_GRAPH
+    capture = TryOnDenoiser.capture
+
+    def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots):
+        self.tryon, self.garment = tryon, garment
+        self.L = tryon.L
+        self.device = tryon.device
+        self.S = int(slots)
+        self._graph = None
+        self._key = None
+        self.ctx_t = None
+
+    def _needs(self, kind):
+        names = ["b200vton_cfg_ddpm_step_rows" if kind == "ddpm" else "b200vton_cfg_solver_step_rows"]
+        if kind == "euler":
+            names.append("b200vton_nchw_to_nhwc_scaled_rows")
+        return names
+
+    def configure(self, scheduler, timesteps, h, w, guidance_scale=2.0, do_cfg=True, eta=0.0, guidance_rescale=0.0):
+        """Per-step tables of the run (one scheduler, one step count for every request) and the static buffers of a
+        person latent size h x w (the garment has the same size). Raises before any launch when the library lacks a
+        per-slot kernel the scheduler needs, and for guidance_rescale > 0 (its per-sample statistics are fused with the
+        single-row DDPM kernel only)."""
+        if guidance_rescale and guidance_rescale > 0:
+            raise NotImplementedError("guidance_rescale > 0 is not supported by continuous batching: the rescale kernel "
+                                      "reads one coefficient row for the whole batch")
+        kind, coefs, scales, self.step_draws, self.noise_applied = solver_step_tables(scheduler, timesteps, eta)
+        for name in self._needs(kind):
+            if not self.L.has_symbol(name):
+                raise NotImplementedError(f"continuous batching needs {name}, which this library binding does not export")
+        gs = float(guidance_scale)
+        rows = [[gs, *c, 0.0, 0.0] if kind == "ddpm" else [gs, *c] for c in coefs]
+        rows.append(identity_step_row(kind))                       # row T: idle slots
+        dev, f16, f32 = self.device, torch.float16, torch.float32
+        self.T = len(coefs)
+        self.coef_table = torch.tensor(rows, dtype=f32, device=dev)
+        self.t_table = torch.tensor([float(t) for t in timesteps] + [0.0], dtype=f32, device=dev)
+        self.scale_table = None if scales is None else torch.tensor(list(scales) + [1.0], dtype=f32, device=dev)
+        self.kind, self.do_cfg, self.h, self.w = kind, bool(do_cfg), h, w
+        S = self.S
+        self.Bt = 2 * S if do_cfg else S
+        key = (S, h, w, self.do_cfg, kind)
+        if key != self._key:
+            self._key = key
+            self._graph = None
+            self.ctx_t = self.ctx_g = self.aug = None
+            self.latents = torch.zeros((S, 4, h, w), dtype=f16, device=dev)
+            self.latents_next = torch.zeros_like(self.latents)
+            self.noise = torch.zeros_like(self.latents)
+            self.x0_prev = torch.zeros_like(self.latents) if kind == "dpmpp" else None
+            self.x_t = torch.zeros((self.Bt, h, w, CIN_PAD), dtype=f16, device=dev)
+            self.x_g = torch.zeros((S, h, w, CIN_PAD), dtype=f16, device=dev)
+            self.t_g = torch.zeros(S, dtype=f32, device=dev)
+            self.t_t = torch.zeros(self.Bt, dtype=f32, device=dev)
+            self.coef = torch.zeros((S, 8), dtype=f32, device=dev)
+            self.scale = torch.ones(S, dtype=f32, device=dev)
+        self.gather([None] * S)
+
+    def gather(self, steps):
+        """steps: per slot, the step index of its request or None (idle). Copies row steps[s] (row T when idle) of the
+        tables into the graph's static t / coef / scale buffers (t at rows s and S + s of the try-on batch)."""
+        idx = torch.tensor([self.T if i is None else int(i) for i in steps], dtype=torch.long).to(self.device)
+        torch.index_select(self.coef_table, 0, idx, out=self.coef)
+        t = self.t_table.index_select(0, idx)
+        self.t_g.copy_(t)
+        self.t_t.copy_(t.repeat(self.Bt // self.S))
+        if self.scale_table is not None:
+            torch.index_select(self.scale_table, 0, idx, out=self.scale)
+
+    def _rows(self, s):
+        return (s, self.S + s) if self.do_cfg else (s,)
+
+    def admit(self, s, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
+              add_time_ids, image_embeds, text_embeds_cloth):
+        """Writes one request into slot s, and only its rows. latents [1,4,h,w]; mask [1,1,h,w]; masked_image_latents,
+        pose_latents, cloth_latents [1,4,h,w]; prompt_embeds [n,77,X], add_text_embeds [n,P], add_time_ids [n,6],
+        image_embeds [n,16,X] with n = 2 ([uncond ; cond]) under CFG, else 1 (mask, masked_image_latents and
+        pose_latents may have n rows too); text_embeds_cloth [1,77,X]."""
+        L, dev, f16 = self.L, self.device, torch.float16
+        for name, t in (("latents", latents), ("mask", mask), ("masked_image_latents", masked_image_latents),
+                        ("pose_latents", pose_latents), ("cloth_latents", cloth_latents)):
+            if tuple(t.shape[-2:]) != (self.h, self.w):
+                raise ValueError(f"{name} has spatial size {tuple(t.shape[-2:])}, the server's latents {(self.h, self.w)}")
+        rows = self._rows(s)
+        if self.ctx_t is None:
+            ni = image_embeds.shape[1] if self.tryon.ip_tokens else 0
+            self.ctx_t = [(torch.zeros((self.Bt, prompt_embeds.shape[1], 2 * b.c), dtype=f16, device=dev),
+                           torch.zeros((self.Bt, ni, 2 * b.c), dtype=f16, device=dev) if ni else None)
+                          for b in self.tryon.blocks()]
+            self.ctx_g = [(torch.zeros((self.S, text_embeds_cloth.shape[1], 2 * b.c), dtype=f16, device=dev), None)
+                          for b in self.garment.blocks()]
+            self.aug = torch.zeros((self.Bt, self.tryon.ae[2].shape[0]), dtype=f16, device=dev)
+            self._graph = None
+        self.latents[s].copy_(latents[0].to(dev, f16))
+        for j, r in enumerate(rows):
+            x = self.x_t[r:r + 1]
+            for t, c_off in ((mask, 4), (masked_image_latents, 5), (pose_latents, 9)):
+                row = t[j:j + 1] if t.shape[0] == len(rows) else t[:1]
+                L.nchw_to_nhwc(row.to(dev, f16).contiguous(), x, c_off=c_off)
+            self.tryon.encode_context(prompt_embeds[j:j + 1].to(dev, f16), image_embeds[j:j + 1].to(dev, f16),
+                                      out=[(kt[r:r + 1], None if ki is None else ki[r:r + 1]) for kt, ki in self.ctx_t])
+            self.tryon.aug_embedding(add_text_embeds[j:j + 1].to(dev, f16), add_time_ids[j:j + 1].to(dev),
+                                     out=self.aug[r:r + 1])
+        L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), self.x_g[s:s + 1], c_off=0)
+        self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16), out=[(kv[s:s + 1], None) for kv, _ in self.ctx_g])
+        if self.x0_prev is not None:
+            self.x0_prev[s].zero_()
+
+    def release(self, s):
+        """Frees slot s: its latents, state and input channels go back to zeros (the context rows keep finite values
+        that no other slot reads)."""
+        for buf in (self.latents, self.latents_next, self.noise, self.x0_prev, self.x_g):
+            if buf is not None:
+                buf[s].zero_()
+        for r in self._rows(s):
+            self.x_t[r].zero_()
+
+    def _launch_step(self):
+        """The launch sequence of one step over the slot buffers (graph-capturable)."""
+        L, S = self.L, self.S
+        if self.kind == "euler":                        # scale_model_input with each slot's own sigma
+            L.nchw_to_nhwc_scaled_rows(self.latents, self.x_t, self.scale, c_off=0)
+        else:
+            L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)
+        feats = []
+        self.garment.forward(self.x_g, self.garment.time_embedding(self.t_g, S), self.ctx_g, collect=feats)
+        temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
+        self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=S if self.do_cfg else 0)
+        if self.kind == "ddpm":
+            L.cfg_ddpm_step_rows(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
+        else:
+            L.cfg_solver_step_rows(self.eps, self.latents, self.noise if self.kind == "ddim" else None, self.coef,
+                                   self.kind, x0_prev=self.x0_prev, do_cfg=self.do_cfg, out=self.latents_next)
+        self.latents.copy_(self.latents_next)
+
+    def step(self, steps, noises=None, use_graph=True):
+        """One denoise step of every occupied slot. steps: per slot, its request's step index or None (idle); noises:
+        {slot: [1,4,h,w] variance noise} for the slots whose scheduler step applies one. Returns the latents [S,4,h,w]."""
+        if self.ctx_t is None:
+            raise RuntimeError("SlotDenoiser.step before any admission")
+        self.gather(steps)
+        self.noise.zero_()
+        for s, n in (noises or {}).items():
+            self.noise[s].copy_(n[0])
+        with nvtx_range("b200vton.slot_denoise_step"):
+            if use_graph:
+                if self._graph is None:
+                    self.capture()
+                self._graph.replay()
+            else:
+                self._launch_step()
+        return self.latents

@@ -47,6 +47,15 @@ SIGNATURES = {
     "b200vton_postprocess_image": [_vp, _i, _i, _i, _i, _vp, _vp, _vp],
 }
 
+# Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
+# step kernels of the continuous-batching denoiser. `has_symbol` tells whether a binding can use them.
+OPTIONAL_SIGNATURES = {
+    "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
+    "b200vton_cfg_solver_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp],
+    "b200vton_nchw_to_nhwc_scaled_rows": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp],
+}
+_present = set()
+
 _lib = None
 ABI_VERSION = 109      # must equal b200vton_version() of the loaded library (bumped with every SIGNATURES change)
 
@@ -95,6 +104,12 @@ def load(build_if_missing=True):
         fn = getattr(lib, name)
         fn.argtypes = args
         fn.restype = _i
+    for name, args in OPTIONAL_SIGNATURES.items():
+        fn = getattr(lib, name, None)
+        if fn is not None:
+            fn.argtypes = args
+            fn.restype = _i
+            _present.add(name)
     _lib = lib
     return lib
 
@@ -115,6 +130,18 @@ def get_option(name, default=0):
 def launch_count():
     """Kernels launched (or captured) by libb200vton.so since load."""
     return int(load().b200vton_launch_count())
+
+
+def has_symbol(name):
+    """Whether the loaded library exports the optional entry point `name` (OPTIONAL_SIGNATURES)."""
+    load()
+    return name in _present
+
+
+def _optional(name):
+    if not has_symbol(name):
+        raise NotImplementedError(f"{LIB_PATH} does not export {name}: rebuild it (python idm-vton_b200/build.py --force)")
+    return getattr(_lib, name)
 
 
 def _check(rc, name):
@@ -607,3 +634,50 @@ def cfg_solver_step(eps, latents, noise, coef, kind, x0_prev=None, do_cfg=True, 
                                       SOLVER_KINDS[kind], int(do_cfg), _p(out), _stream())
     _check(rc, "b200vton_cfg_solver_step")
     return out
+
+
+def _coef_rows(coef, B, name):
+    """coef: [B, stride] fp32 CUDA rows (contiguous) or one row [n] shared by all samples (stride 0)."""
+    if coef.dtype != torch.float32 or not coef.is_cuda or not coef.is_contiguous():
+        raise TypeError(f"{name}: coef must be a contiguous CUDA fp32 tensor")
+    if coef.dim() == 1:
+        return 0
+    if coef.dim() != 2 or coef.shape[0] != B:
+        raise ValueError(f"{name}: coef must be [B={B}, stride] or one row, got {tuple(coef.shape)}")
+    return coef.shape[1]
+
+
+def cfg_ddpm_step_rows(eps, latents, noise, coef, do_cfg=True, out=None):
+    """cfg_ddpm_step with one coefficient row per sample: coef [B, stride >= 6] fp32 on device, sample b reads row b."""
+    fn = _optional("b200vton_cfg_ddpm_step_rows")
+    B, C, H, W = latents.shape
+    stride = _coef_rows(coef, B, "cfg_ddpm_step_rows")
+    if out is None:
+        out = torch.empty_like(latents)
+    rc = fn(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(coef), stride, int(do_cfg), _p(out), _stream())
+    _check(rc, "b200vton_cfg_ddpm_step_rows")
+    return out
+
+
+def cfg_solver_step_rows(eps, latents, noise, coef, kind, x0_prev=None, do_cfg=True, out=None):
+    """cfg_solver_step with one coefficient row per sample: coef [B, stride >= 8] fp32 on device, sample b reads row b."""
+    fn = _optional("b200vton_cfg_solver_step_rows")
+    B, C, H, W = latents.shape
+    stride = _coef_rows(coef, B, "cfg_solver_step_rows")
+    if out is None:
+        out = torch.empty_like(latents)
+    rc = fn(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(x0_prev), _p(coef), stride,
+            SOLVER_KINDS[kind], int(do_cfg), _p(out), _stream())
+    _check(rc, "b200vton_cfg_solver_step_rows")
+    return out
+
+
+def nchw_to_nhwc_scaled_rows(src, dst, scale, c_off=0):
+    """nchw_to_nhwc with dst row s = fp16(src[s % Bs] * scale[s % Bs]); scale: Bs fp32 on the device."""
+    _check_scatter_shapes(src, dst, c_off)
+    fn = _optional("b200vton_nchw_to_nhwc_scaled_rows")
+    Bs, Cs, H, W = src.shape
+    assert scale.dtype == torch.float32 and scale.is_cuda and scale.numel() >= Bs
+    rc = fn(_p(src), Bs, Cs, H, W, _p(dst), dst.shape[0], dst.shape[-1], c_off, _p(scale), _stream())
+    _check(rc, "b200vton_nchw_to_nhwc_scaled_rows")
+    return dst

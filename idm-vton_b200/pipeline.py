@@ -554,6 +554,37 @@ class StableDiffusionXLInpaintPipeline:
                              "`text_encoder_2.config.projection_dim`.")
         return torch.tensor([add_time_ids], dtype=dtype), torch.tensor([add_neg_time_ids], dtype=dtype)
 
+    def _preprocess_image_mask(self, image, mask_image, masked_image_latents, height, width):
+        """Step 5 of __call__ (src/tryon_pipeline.py:1588-1602): (init_image, mask, masked_image, mask_latent); mask_latent
+        is the latent-resolution mask when the one-launch kernel made it, else None."""
+        if masked_image_latents is None and self._fused_preprocess_ok(image, mask_image, height, width):
+            # GPU tensors at the target size: image normalisation, mask grayscale + binarisation, the masked image and the
+            # latent-resolution mask in ONE launch (b200vton_preprocess_inpaint; same arithmetic as the two
+            # VaeImageProcessor.preprocess calls below + :1598 + the nearest resize of :940-943)
+            from . import lib as L
+            return L.preprocess_inpaint(image.to(torch.float32).contiguous(), mask_image.to(torch.float32).contiguous(),
+                                        self.vae_scale_factor)
+        init_image = self.image_processor.preprocess(image, height=height, width=width).to(dtype=torch.float32)
+        mask = self.mask_processor.preprocess(mask_image, height=height, width=width)
+        if masked_image_latents is not None:
+            masked_image = masked_image_latents
+        elif init_image.shape[1] == 4:
+            masked_image = None
+        else:
+            masked_image = init_image * (mask.to(init_image.device) < 0.5)
+        return init_image, mask, masked_image, None
+
+    def _pose_latents(self, pose_img, dtype):
+        """src/tryon_pipeline.py:1646: the pose image's posterior sample, drawn from the GLOBAL generator."""
+        pose_img = self.vae.encode(pose_img.to(self.vae.dtype)).latent_dist.sample().to(dtype)
+        return pose_img * self.vae.config.scaling_factor
+
+    def _decode_latents(self, latents):
+        """src/tryon_pipeline.py:1868-1880: the VAE decode (fp32 twin when the fp16 VAE asks for upcasting)."""
+        needs_upcasting = self.vae.dtype == torch.float16 and self.vae.config.force_upcast
+        vae = self._vae32() if needs_upcasting else self.vae
+        return vae.decode(latents.to(vae.dtype) / self.vae.config.scaling_factor, return_dict=False)[0]
+
     # ---------------------------------------------------------------------------------------------
     @torch.no_grad()
     def __call__(
@@ -662,23 +693,8 @@ class StableDiffusionXLInpaintPipeline:
         if trace:
             trace.mark("prompt+timesteps")
         # 5. image / mask
-        mask_latent = None
-        if masked_image_latents is None and self._fused_preprocess_ok(image, mask_image, height, width):
-            # GPU tensors at the target size: image normalisation, mask grayscale + binarisation, the masked image and the
-            # latent-resolution mask in ONE launch (b200vton_preprocess_inpaint; same arithmetic as the two
-            # VaeImageProcessor.preprocess calls below + :1598 + the nearest resize of :940-943)
-            from . import lib as L
-            init_image, mask, masked_image, mask_latent = L.preprocess_inpaint(
-                image.to(torch.float32).contiguous(), mask_image.to(torch.float32).contiguous(), self.vae_scale_factor)
-        else:
-            init_image = self.image_processor.preprocess(image, height=height, width=width).to(dtype=torch.float32)
-            mask = self.mask_processor.preprocess(mask_image, height=height, width=width)
-            if masked_image_latents is not None:
-                masked_image = masked_image_latents
-            elif init_image.shape[1] == 4:
-                masked_image = None
-            else:
-                masked_image = init_image * (mask.to(init_image.device) < 0.5)
+        init_image, mask, masked_image, mask_latent = self._preprocess_image_mask(image, mask_image, masked_image_latents,
+                                                                                  height, width)
 
         # 6. latents (RNG draw #1; with strength < 1 the image-latents sample comes first, then the noise)
         num_channels_latents = self.vae.config.latent_channels
@@ -720,8 +736,7 @@ class StableDiffusionXLInpaintPipeline:
             mask, masked_image_latents = self.prepare_mask_latents(mask, masked_image, batch_size * num_images_per_prompt,
                                                                    height, width, prompt_embeds.dtype, device, generator,
                                                                    self.do_classifier_free_guidance, _mask_latent=mask_latent)
-            pose_img = self.vae.encode(pose_img.to(self.vae.dtype)).latent_dist.sample().to(prompt_embeds.dtype)
-            pose_img = pose_img * self.vae.config.scaling_factor
+            pose_img = self._pose_latents(pose_img, prompt_embeds.dtype)
             pose_img = torch.cat([pose_img] * 2) if self.do_classifier_free_guidance else pose_img
             if cloth_is_latents:
                 # extension: already-encoded (and scaled) garment latents, as image / masked_image_latents may be
@@ -812,9 +827,7 @@ class StableDiffusionXLInpaintPipeline:
             trace.mark("denoise loop")
 
         if not output_type == "latent":
-            needs_upcasting = self.vae.dtype == torch.float16 and self.vae.config.force_upcast
-            vae = self._vae32() if needs_upcasting else self.vae
-            image = vae.decode(latents.to(vae.dtype) / self.vae.config.scaling_factor, return_dict=False)[0]
+            image = self._decode_latents(latents)
         # NB (reference quirk, src/tryon_pipeline.py:1868-1885): with output_type == "latent", `image` is still the
         # caller's input image, and that is what gets returned.
         image = self._postprocess(image, output_type)

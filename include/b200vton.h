@@ -155,6 +155,11 @@ int b200vton_nchw_to_nhwc(const void* src, int Bs, int Cs, int H, int W, void* d
  * (src/tryon_pipeline.py:1772, before the channel concat of :1777). */
 int b200vton_nchw_to_nhwc_scaled(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,
                                  const void* scale, void* stream);
+/* b200vton_nchw_to_nhwc_scaled with one scale per source sample: dst[s, ..] = fp16(src[s % Bs, ..] * scale[s % Bs]);
+ * scale: Bs fp32 on device. Rows b and b + Bs of the CFG duplication both use scale[b]: Euler's scale_model_input when
+ * every sample is at its own step (continuous batching). Pointers not null; src / dst 2-byte, scale 4-byte aligned. */
+int b200vton_nchw_to_nhwc_scaled_rows(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc,
+                                      int c_off, const void* scale, void* stream);
 /* dst NCHW [B,C,H,W] = src NHWC [B,H,W,ldc][..., :C] */
 int b200vton_nhwc_to_nchw(const void* src, int B, int C, int H, int W, int ldc, void* dst, void* stream);
 
@@ -222,6 +227,18 @@ int b200vton_cfg_rescale_ddpm_step(const void* eps, int ldc, int B, int C, int H
 int b200vton_cfg_solver_step(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
                              const void* noise, void* x0_prev, const void* coef, int kind, int do_cfg, void* out,
                              void* stream);
+
+/* b200vton_cfg_ddpm_step / b200vton_cfg_solver_step with one coefficient row per sample: coef is [B, coef_stride] fp32 on
+ * device and sample b reads row b, so every sample of the batch can be at its own denoise step (continuous batching).
+ * coef_stride 0 gives every sample row 0, which is the single-row entry point's result bit for bit; otherwise it must be
+ * at least the kind's coefficient count (6 for DDPM, 8 for the solver kinds). Same layouts and rounding points as the
+ * single-row entry points; eps, latents, coef and out not null; fp16 pointers 2-byte aligned, coef 4-byte. */
+int b200vton_cfg_ddpm_step_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                const void* noise, const void* coef, int coef_stride, int do_cfg, void* out,
+                                void* stream);
+int b200vton_cfg_solver_step_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                  const void* noise, void* x0_prev, const void* coef, int coef_stride, int kind,
+                                  int do_cfg, void* out, void* stream);
 
 /* Pre-processing of the inpainting inputs in one launch (diffusers VaeImageProcessor.preprocess for image and mask,
  * the masked image and the latent-resolution mask: src/tryon_pipeline.py:1588-1602, 940-943). image: [B,3,H,W] fp32;
