@@ -5,11 +5,15 @@
 //            (K1/K2/K5: ResnetBlock2D conv1/conv2/conv_shortcut, conv_in, conv_out; NHWC, pad 1, stride 1 or 2)
 //   fp32 conv3x3 (the VAE): TF32 operands (or fp16 operands) with fp32 accumulate, bias, residual and output.
 //
-// One CTA computes one 128 x BN output tile. Warps 0..7 are two consumer warpgroups (rows 0..63 / 64..127 of the tile)
-// that issue m64nBNk16 (k8 for TF32) wgmma from 128B-swizzled shared memory into register accumulators; warp 8 is the
-// TMA producer. The conv walks K as 9 taps x Cin/64 slabs with a 4-D tensor map over [B,H,W,C]; out-of-bounds box
-// elements are zero-filled by TMA, which is the conv's zero padding. After the K loop the accumulators are staged as fp32
-// in shared memory (the operand ring is dead by then) and every thread runs the fused epilogue for one row.
+// A CTA computes 128 x BN output tiles, one after another: the grid is min(tiles, SMs) and CTA b takes tiles b,
+// b + gridDim.x, ... (n fastest, so neighbouring CTAs share an A slab in L2). Warps 0..7 are two consumer warpgroups
+// (rows 0..63 / 64..127 of the tile) that issue m64nBNk16 (k8 for TF32) wgmma from 128B-swizzled shared memory into
+// register accumulators; warp 8 (in a warpgroup of its own, which gives its registers to the consumers) is the TMA
+// producer. The conv walks K as 9 taps x Cin/64 slabs with a 4-D tensor map over [B,H,W,C]; out-of-bounds box elements
+// are zero-filled by TMA, which is the conv's zero padding. After a tile's K loop each consumer thread runs the fused
+// epilogue on its own accumulator fragment (gemm_common.cuh) and stores 16 bytes at a time. The epilogue does not touch
+// shared memory, so the producer runs on into the next tile's slabs meanwhile and the operand ring is full again when
+// the consumers come back: only a CTA's first tile waits for a load.
 // Epilogue rounding points replicate the reference's fp16-autocast path (SURVEY.md App. D.1):
 //   v = fp16(acc + bias); v = fp16(v + temb[b,n]); s = fp16(acc_sc + bias_sc); v = fp16(s + v); v = fp16(v + res)
 #include "gemm_common.cuh"
@@ -20,52 +24,37 @@ namespace vton {
 
 enum : int { KIND_F16 = 0, KIND_F16IN_F32OUT = 1, KIND_TF32 = 2 };
 
-template <int BN, int STAGES, bool SC>
+template <int BN, int STAGES>
 struct SmemLayout {
   static constexpr int B_BYTES = BN * 128;              // BN rows x 128 B (64 halves or 32 floats)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int LDS = BN + 4;                    // staging row stride in floats (bank spread, 16-byte rows)
-  static constexpr int STG_BYTES = 128 * LDS * 4;
-  static constexpr int RING = STAGES * STAGE_BYTES;
-  static constexpr int STG_TOTAL = (SC ? 2 : 1) * STG_BYTES;
-  static constexpr int BAR_OFFSET = RING > STG_TOTAL ? RING : STG_TOTAL;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // barriers + alignment slack
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;   // the barriers follow the operand ring
+  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;     // barriers + alignment slack
 };
 
-constexpr int GEMM_THREADS = 288;   // 2 consumer warpgroups + 1 producer warp
+// 2 consumer warpgroups + the producer's warpgroup (warp 8 loads; warps 9..11 only hand over their registers). ptxas
+// allots registers per whole warpgroup, 65536 / 384 = 168 a thread, which does not hold a 128-float accumulator and the
+// epilogue; so the producer's warpgroup drops to 40 and the consumers rise to 232 (128 * 40 + 256 * 232 <= 65536).
+constexpr int GEMM_THREADS = 384;
+constexpr int GEMM_PRODUCER_REGS = 40;
+constexpr int GEMM_CONSUMER_REGS = 232;
 
 template <int BN, int STAGES, bool GEGLU, bool SC, int KIND>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmS0, const __grid_constant__ CUtensorMap tmS1,
                  const __grid_constant__ CUtensorMap tmBs, const GemmParams p) {
-  using L = SmemLayout<BN, STAGES, SC>;
+  using L = SmemLayout<BN, STAGES>;
   constexpr int KBK = KIND == KIND_TF32 ? 32 : 64;   // channels per 128-byte slab row
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  float* stg = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int tile = blockIdx.x;
-  const int n_tile = tile % p.n_tiles;
-  const int m_tile = tile / p.n_tiles;
-  const int n0 = n_tile * BN;
   const int total_slabs = p.slabs_main + (SC ? p.slabs_sc : 0);
-
-  // conv tile origin
-  int b0 = 0, y0 = 0, x0 = 0;
-  if (p.conv) {
-    const int tx = m_tile % p.tiles_x;
-    const int ty = (m_tile / p.tiles_x) % p.tiles_y;
-    const int tb = m_tile / (p.tiles_x * p.tiles_y);
-    x0 = tx * p.bw;
-    y0 = ty * p.bh;
-    b0 = tb * p.bb;
-  }
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -85,34 +74,48 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   __syncthreads();
   pdl_launch_dependents();
 
-  if (warp == 8) {
+  // The producer and both consumer warpgroups walk the same static tile schedule, and each keeps one slab counter `it`
+  // that runs on across tiles: slab `it` lives in stage it % STAGES on barrier phase (it / STAGES) & 1.
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int s = 0; s < total_slabs; ++s) {
-        const int stage = s % STAGES;
-        const uint32_t phase = (s / STAGES) & 1;
-        mbar_wait(empty_bar(stage), phase ^ 1);
-        const uint32_t a_dst = smem_base + stage * L::STAGE_BYTES;
-        const uint32_t b_dst = a_dst + A_BYTES;
-        mbar_expect_tx(full_bar(stage), L::STAGE_BYTES);
-        if (s < p.slabs_main) {
-          if (p.conv) {
-            const int tap = s / p.cin_slabs;
-            const int c0 = (s - tap * p.cin_slabs) * KBK;
-            const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-            tma_load_4d(a_dst, &tmA, full_bar(stage), c0, x0 * p.stride + dx, y0 * p.stride + dy, b0);
-            tma_load_2d(b_dst, &tmB, full_bar(stage), c0, tap * p.cout + n0);
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int n0 = (tile % p.n_tiles) * BN;
+        const int m_tile = tile / p.n_tiles;
+        int b0 = 0, y0 = 0, x0 = 0;   // conv tile origin
+        if (p.conv) {
+          x0 = (m_tile % p.tiles_x) * p.bw;
+          y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.bh;
+          b0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.bb;
+        }
+        for (int s = 0; s < total_slabs; ++s, ++it) {
+          const int stage = it % STAGES;
+          const uint32_t phase = (it / STAGES) & 1;
+          mbar_wait(empty_bar(stage), phase ^ 1);
+          const uint32_t a_dst = smem_base + stage * L::STAGE_BYTES;
+          const uint32_t b_dst = a_dst + A_BYTES;
+          mbar_expect_tx(full_bar(stage), L::STAGE_BYTES);
+          if (s < p.slabs_main) {
+            if (p.conv) {
+              const int tap = s / p.cin_slabs;
+              const int c0 = (s - tap * p.cin_slabs) * KBK;
+              const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+              tma_load_4d(a_dst, &tmA, full_bar(stage), c0, x0 * p.stride + dx, y0 * p.stride + dy, b0);
+              tma_load_2d(b_dst, &tmB, full_bar(stage), c0, tap * p.cout + n0);
+            } else {
+              tma_load_2d(a_dst, &tmA, full_bar(stage), s * KBK, m_tile * BM);
+              tma_load_2d(b_dst, &tmB, full_bar(stage), s * KBK, n0);
+            }
           } else {
-            tma_load_2d(a_dst, &tmA, full_bar(stage), s * KBK, m_tile * BM);
-            tma_load_2d(b_dst, &tmB, full_bar(stage), s * KBK, n0);
+            const int ss = s - p.slabs_main;
+            if (ss < p.sc_split)
+              tma_load_4d(a_dst, &tmS0, full_bar(stage), ss * BK, x0, y0, b0);
+            else
+              tma_load_4d(a_dst, &tmS1, full_bar(stage), (ss - p.sc_split) * BK, x0, y0, b0);
+            tma_load_2d(b_dst, &tmBs, full_bar(stage), ss * BK, n0);
           }
-        } else {
-          const int ss = s - p.slabs_main;
-          if (ss < p.sc_split)
-            tma_load_4d(a_dst, &tmS0, full_bar(stage), ss * BK, x0, y0, b0);
-          else
-            tma_load_4d(a_dst, &tmS1, full_bar(stage), (ss - p.sc_split) * BK, x0, y0, b0);
-          tma_load_2d(b_dst, &tmBs, full_bar(stage), ss * BK, n0);
         }
       }
     }
@@ -120,15 +123,24 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 
   // ===================== consumers: two warpgroups, 64 accumulator rows each =====================
+  setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   const int wg = warp >> 2;
+  const int r_local = wg * 64 + ((warp & 3) << 4) + (lane >> 2);   // the thread's first fragment row (the other: + 8)
   float acc[BN / 2];
   float acc_sc[BN / 2];   // shortcut accumulator (dead when !SC)
-  // One K slab per iteration; slabs [s_begin, s_end) accumulate into accr (a separate loop per accumulator keeps the
-  // choice of registers static, so the wgmma pipeline is not serialised).
+  uint32_t it = 0;
+  // Every slab is released (one arrival per warpgroup on its stage's empty barrier) exactly once, after the wgmma wait
+  // that retires it: slab it - 1 after the wait<1> that follows slab it's commit, a tile's last slab after the wait<0>
+  // that ends the tile.
+  auto release = [&](uint32_t slab) {
+    if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(slab % STAGES));
+  };
+  // One K slab per iteration; slabs [s_begin, s_end) of the tile accumulate into accr (a separate loop per accumulator
+  // keeps the choice of registers static, so the wgmma pipeline is not serialised).
   auto run_slabs = [&](float (&accr)[BN / 2], int s_begin, int s_end) {
-    for (int s = s_begin; s < s_end; ++s) {
-      const int stage = s % STAGES;
-      mbar_wait(full_bar(stage), (s / STAGES) & 1);
+    for (int s = s_begin; s < s_end; ++s, ++it) {
+      const int stage = it % STAGES;
+      mbar_wait(full_bar(stage), (it / STAGES) & 1);
       const uint32_t a_src = smem_base + stage * L::STAGE_BYTES + wg * (64 * 128);
       const uint32_t b_src = smem_base + stage * L::STAGE_BYTES + A_BYTES;
       wgmma_fence();
@@ -144,61 +156,23 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
       wgmma_commit();
-      wgmma_wait<1>();   // the previous slab's MMAs have retired: its stage may be refilled
-      if (s > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar((s - 1) % STAGES));
+      wgmma_wait<1>();
+      if (s > 0) release(it - 1);   // s == 0: the previous slab was the last of the tile before and is released already
     }
   };
-  run_slabs(acc, 0, p.slabs_main);
-  if constexpr (SC) run_slabs(acc_sc, p.slabs_main, total_slabs);
-  wgmma_wait<0>();
-  fence_regs(acc);
-  if (SC) fence_regs(acc_sc);
-
-  // ===================== epilogue: registers -> fp32 staging tile -> fused epilogue, one row per thread =====================
-  named_bar_sync(1, 256);   // both warpgroups are done reading the operand ring
-  {
-    const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
-    const int cq = (lane & 3) * 2;
-#pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-      *reinterpret_cast<float2*>(stg + r0 * L::LDS + i * 8 + cq) = make_float2(acc[4 * i], acc[4 * i + 1]);
-      *reinterpret_cast<float2*>(stg + (r0 + 8) * L::LDS + i * 8 + cq) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-      if (SC) {
-        float* s2 = stg + 128 * L::LDS;
-        *reinterpret_cast<float2*>(s2 + r0 * L::LDS + i * 8 + cq) = make_float2(acc_sc[4 * i], acc_sc[4 * i + 1]);
-        *reinterpret_cast<float2*>(s2 + (r0 + 8) * L::LDS + i * 8 + cq) = make_float2(acc_sc[4 * i + 2], acc_sc[4 * i + 3]);
-      }
-    }
-  }
-  named_bar_sync(1, 256);
-  const int row = threadIdx.x & 127;
-  const int half = threadIdx.x >> 7;
-  long long out_row;
-  int sample;
-  map_row(p, m_tile, row, &out_row, &sample);
-  const float* srow = stg + row * L::LDS;
-  if (KIND == KIND_F16) {
-    epilogue_store<BN, GEGLU>(p, srow, SC ? srow + 128 * L::LDS : nullptr, n_tile, out_row, sample, half, 2);
-    return;
-  }
-  if (out_row < 0) return;
-  const float* res_row = p.res_f32 ? p.res_f32 + out_row * p.N : nullptr;
-#pragma unroll 1
-  for (int c = half; c < BN / 32; c += 2) {
-    const int ncol = n0 + c * 32;
-    if (ncol >= p.N) continue;
-#pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      float4 v = *reinterpret_cast<const float4*>(srow + c * 32 + g * 4);
-      if (p.bias_f32 != nullptr) {
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias_f32 + ncol + g * 4));
-        v.x += b4.x, v.y += b4.y, v.z += b4.z, v.w += b4.w;
-      }
-      if (res_row != nullptr) {   // after the bias, like torch's `x + conv(h)`
-        const float4 r4 = __ldg(reinterpret_cast<const float4*>(res_row + ncol + g * 4));
-        v.x += r4.x, v.y += r4.y, v.z += r4.z, v.w += r4.w;
-      }
-      *reinterpret_cast<float4*>(p.out_f32 + out_row * p.N + ncol + g * 4) = v;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    EpilogueF16<BN, GEGLU, SC> epi;   // fp16 kinds: the tile's bias and first residual loads fly during the K loop
+    if constexpr (KIND == KIND_F16) epi.begin(p, tile / p.n_tiles, tile % p.n_tiles, r_local);
+    run_slabs(acc, 0, p.slabs_main);
+    if constexpr (SC) run_slabs(acc_sc, p.slabs_main, total_slabs);
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (SC) fence_regs(acc_sc);
+    release(it - 1);
+    if constexpr (KIND == KIND_F16) {
+      epi.finish(p, acc, acc_sc);
+    } else {
+      epilogue_f32<BN>(p, tile / p.n_tiles, tile % p.n_tiles, r_local, acc);
     }
   }
 }
@@ -208,9 +182,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // ------------------------------------------------------------------------------------------------
 template <int BN, int STAGES, bool GEGLU, bool SC, int KIND>
 static int launch_variant(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmS0,
-                          const CUtensorMap& tmS1, const CUtensorMap& tmBs, const GemmParams& p, int grid,
-                          cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES, SC>;
+                          const CUtensorMap& tmS1, const CUtensorMap& tmBs, const GemmParams& p, cudaStream_t stream) {
+  using L = SmemLayout<BN, STAGES>;
   static_assert(L::TOTAL <= 227 * 1024, "shared memory budget");
   auto kern = gemm_conv_kernel<BN, STAGES, GEGLU, SC, KIND>;
   static bool configured = false;
@@ -218,6 +191,7 @@ static int launch_variant(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
     VTON_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     configured = true;
   }
+  const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();   // every CTA loops over its share of the tiles
   VTON_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), L::TOTAL, stream, tmA, tmB, tmS0, tmS1, tmBs, p));
   count_launch();
   return kOk;
@@ -267,25 +241,25 @@ static int dispatch(int bn, bool geglu, const CUtensorMap& tmA, const CUtensorMa
                     const CUtensorMap& tmS1, const CUtensorMap& tmBs, GemmParams& p, int m_tiles,
                     cudaStream_t stream) {
   p.n_tiles = cdiv(p.N, bn);
-  const int grid = m_tiles * p.n_tiles;
+  p.total_tiles = m_tiles * p.n_tiles;
   if (geglu) {
-    if (bn == 128) return launch_variant<128, 6, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    if (bn == 256) return launch_variant<256, 4, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
+    if (bn == 128) return launch_variant<128, 6, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    if (bn == 256) return launch_variant<256, 4, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
     set_last_error("GEGLU epilogue supports BN 128/256 only (got %d)", bn);
     return kErrUnsupported;
   }
   if (p.slabs_sc) {
-    if (bn == 64) return launch_variant<64, 8, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    if (bn == 128) return launch_variant<128, 6, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
+    if (bn == 64) return launch_variant<64, 8, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    if (bn == 128) return launch_variant<128, 6, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
     set_last_error("shortcut epilogue supports BN 64/128 only (got %d)", bn);
     return kErrUnsupported;
   }
   switch (bn) {
-    case 64: return launch_variant<64, 8, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    case 128: return launch_variant<128, 6, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    case 160: return launch_variant<160, 5, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    case 192: return launch_variant<192, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
-    case 256: return launch_variant<256, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, grid, stream);
+    case 64: return launch_variant<64, 8, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 128: return launch_variant<128, 6, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 160: return launch_variant<160, 5, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 192: return launch_variant<192, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 256: return launch_variant<256, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
   }
   set_last_error("unsupported BN %d", bn);
   return kErrUnsupported;
@@ -492,13 +466,13 @@ int conv3x3_f32_impl(const void* x, int B, int H, int W, int Cin, const void* w,
   p.cin_slabs = Cin / bk;
   p.cout = Cout;
   p.n_tiles = cdiv(Cout, bn);
-  const int grid = m_tiles * p.n_tiles;
+  p.total_tiles = m_tiles * p.n_tiles;
   if (in_fp16) {
-    if (bn == 256) return launch_variant<256, 4, false, false, KIND_F16IN_F32OUT>(tmA, tmB, tmA, tmA, tmB, p, grid, stream);
-    return launch_variant<128, 6, false, false, KIND_F16IN_F32OUT>(tmA, tmB, tmA, tmA, tmB, p, grid, stream);
+    if (bn == 256) return launch_variant<256, 4, false, false, KIND_F16IN_F32OUT>(tmA, tmB, tmA, tmA, tmB, p, stream);
+    return launch_variant<128, 6, false, false, KIND_F16IN_F32OUT>(tmA, tmB, tmA, tmA, tmB, p, stream);
   }
-  if (bn == 256) return launch_variant<256, 4, false, false, KIND_TF32>(tmA, tmB, tmA, tmA, tmB, p, grid, stream);
-  return launch_variant<128, 6, false, false, KIND_TF32>(tmA, tmB, tmA, tmA, tmB, p, grid, stream);
+  if (bn == 256) return launch_variant<256, 4, false, false, KIND_TF32>(tmA, tmB, tmA, tmA, tmB, p, stream);
+  return launch_variant<128, 6, false, false, KIND_TF32>(tmA, tmB, tmA, tmA, tmB, p, stream);
 }
 
 }  // namespace vton

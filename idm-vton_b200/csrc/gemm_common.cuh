@@ -1,5 +1,5 @@
 // Shared pieces of the wgmma GEMM / implicit-conv kernel (gemm.cu): the problem descriptor, the accumulator-row ->
-// output-row mapping and the fused epilogue.
+// output-row mapping and the fused epilogue that runs on the accumulator fragments.
 #pragma once
 #include "common.cuh"
 
@@ -27,6 +27,7 @@ struct GemmParams {
   int cin_slabs;  // Cin / 64
   int cout;       // rows per tap in the packed weight
   int n_tiles;
+  int total_tiles;  // m tiles x n_tiles; tile t is (m_tile, n_tile) = (t / n_tiles, t % n_tiles)
   int act_gelu;  // v = fp16(act(fp16(acc + bias))) before the later epilogue terms; 1 = erf-GELU (Resampler FeedForward, CLIP
                  // ViT-H / bigG MLPs), 2 = quick-GELU (CLIP ViT-L text MLP)
   int stride;    // conv: input pixel step per output pixel (1, or 2 = Downsample2D: the A map steps by 2 pixels per row)
@@ -60,10 +61,6 @@ __device__ __forceinline__ void map_row(const GemmParams& p, int m_tile, int r_l
   }
 }
 
-// Epilogue specialisation (compile time): which terms exist. EPI_RUNTIME keeps every term behind a runtime test of the
-// GemmParams pointers.
-enum : int { EPI_BIAS = 1, EPI_ROWVEC = 2, EPI_RES = 4, EPI_RUNTIME = 8 };
-
 // erf-GELU with the Abramowitz-Stegun 7.1.26 rational/exponential form (|abs err| < 2e-7, far below the fp16 rounding
 // that follows): ~16 instructions instead of erff's ~40.
 __device__ __forceinline__ float gelu_erf_fast(float x) {
@@ -82,187 +79,192 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   return 0.5f * x * (1.0f + erf_v);
 }
 
-// chunk c of one accumulator row from the fp32 staging tile in shared memory: accumulator 0 into acc, the gate half /
-// shortcut accumulator into acc2
-template <int BN, bool GEGLU, int EPI>
-__device__ __forceinline__ void epilogue_load(const GemmParams& p, const float* row, const float* row_sc, int c,
-                                              uint32_t (&acc)[32], uint32_t (&acc2)[32]) {
-#pragma unroll
-  for (int i = 0; i < 32; i += 4) {
-    const float4 v = *reinterpret_cast<const float4*>(row + c * 32 + i);
-    acc[i] = __float_as_uint(v.x), acc[i + 1] = __float_as_uint(v.y), acc[i + 2] = __float_as_uint(v.z), acc[i + 3] = __float_as_uint(v.w);
+// Transposes a 4x4 block of words across a quad (lanes 4k .. 4k+3, q = lane & 3): afterwards w[j] of lane q is what
+// lane j held in w[q]. Two exchange rounds (lane bit 0 with index bit 0, then bit 1 with bit 1). Every lane of the warp
+// must call it.
+__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int q) {
+  {
+    const bool odd = (q & 1) != 0;
+    const uint32_t s0 = __shfl_xor_sync(0xffffffffu, odd ? w[0] : w[1], 1);
+    const uint32_t s1 = __shfl_xor_sync(0xffffffffu, odd ? w[2] : w[3], 1);
+    if (odd) w[0] = s0, w[2] = s1;
+    else w[1] = s0, w[3] = s1;
   }
-  const float* src2 = GEGLU ? row + BN / 2 : (((EPI & EPI_RUNTIME) && p.slabs_sc) ? row_sc : nullptr);
-  if (src2 != nullptr) {
+  {
+    const bool hi = (q & 2) != 0;
+    const uint32_t s0 = __shfl_xor_sync(0xffffffffu, hi ? w[0] : w[2], 2);
+    const uint32_t s1 = __shfl_xor_sync(0xffffffffu, hi ? w[1] : w[3], 2);
+    if (hi) w[0] = s0, w[1] = s1;
+    else w[2] = s0, w[3] = s1;
+  }
+}
+
+__device__ __forceinline__ float2 ldg_h2(const __half* src) {
+  return unpack_h2(__ldg(reinterpret_cast<const uint32_t*>(src)));
+}
+
+// Fused fp16 epilogue of one 128 x BN tile, straight from the wgmma accumulator fragment. The thread holds rows r_local
+// and r_local + 8 of the tile and, of every 8-column group i, columns 8i + 2q + {0,1} in acc[4i .. 4i+3] (q = lane & 3);
+// acc_sc (the shortcut accumulator) has the same layout, and the GEGLU gate of column c is column c + BN/2 of the same
+// thread. Per element, with the reference's fp16 rounding points:
+//   v = fp16(acc + bias); v = act(v); v = fp16(v + temb[sample]); v = fp16(fp16(acc_sc + bias_sc) + v); v = fp16(v + res)
+//   GEGLU: v = fp16(h) * fp16(gelu(fp16(g)))
+// Bias and time embedding are read in the fragment shape (one half2 per column pair, the bias once for both rows). The
+// packed half2 words of four 8-groups are then transposed across the quad, so each lane owns 8 contiguous columns of
+// one row: the residual is added and the result stored 16 bytes per lane, a quad filling 64 contiguous bytes of a row.
+// Column groups at or past N and rows outside the output are neither read nor stored.
+//
+// Only eight consumer warps share an SM, so a global load whose value is needed at once costs its whole latency, and a
+// load cannot be moved above an earlier store to `out` by the compiler (the two may alias). begin() therefore runs
+// before the tile's K loop: it maps the rows and issues the loads of the tile's bias words and of the first RES_AHEAD
+// chunks of the residual, which land while the tensor cores work. finish() runs after the K loop and keeps the residual
+// RES_AHEAD chunks ahead of the chunk it stores; a consumed chunk frees 16 accumulator registers for the 8 it loads.
+template <int BN, bool GEGLU, bool SC>
+struct EpilogueF16 {
+  static constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
+  static constexpr int CHUNKS = OUT_COLS / 32;
+  static constexpr bool HAS_RES = !GEGLU && !SC;   // a residual comes with neither GEGLU nor a fused shortcut
+  static constexpr int RES_AHEAD = !HAS_RES ? 1 : (CHUNKS < 4 ? CHUNKS : 4);
+
+  int q, n0, out_n0, out_N;
+  long long out_row[2];
+  int sample[2];
+  uint32_t bias[BN / 8];              // half2 of columns n0 + 8i + 2q + {0,1} (GEGLU: value and gate halves alike)
+  uint32_t bias_sc[SC ? BN / 8 : 1];
+  uint4 res[2][RES_AHEAD];            // residual of chunk c in slot c % RES_AHEAD, in the transposed (stored) shape
+
+  __device__ __forceinline__ int own_col(int c) const { return out_n0 + (4 * c + q) * 8; }   // this lane's 8-group of chunk c
+
+  __device__ __forceinline__ void load_res(const GemmParams& p, int c) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      const float4 v = *reinterpret_cast<const float4*>(src2 + c * 32 + i);
-      acc2[i] = __float_as_uint(v.x), acc2[i + 1] = __float_as_uint(v.y), acc2[i + 2] = __float_as_uint(v.z), acc2[i + 3] = __float_as_uint(v.w);
+    for (int h = 0; h < 2; ++h) {
+      uint4 u = make_uint4(0u, 0u, 0u, 0u);
+      if (p.residual && out_row[h] >= 0 && own_col(c) < out_N)
+        u = *reinterpret_cast<const uint4*>(p.residual + out_row[h] * p.ld_res + own_col(c));
+      res[h][c % RES_AHEAD] = u;
     }
   }
-}
 
-__device__ __forceinline__ void add_h8(float (&v)[8], const __half* src) {
-  const uint4 u = *reinterpret_cast<const uint4*>(src);
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+  __device__ __forceinline__ void begin(const GemmParams& p, int m_tile, int n_tile, int r_local) {
+    q = threadIdx.x & 3;
+    n0 = n_tile * BN;
+    out_n0 = GEGLU ? n_tile * (BN / 2) : n0;
+    out_N = GEGLU ? p.N / 2 : p.N;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 a = unpack_h2(w[j]);
-    v[2 * j] += a.x;
-    v[2 * j + 1] += a.y;
-  }
-}
-__device__ __forceinline__ void add_u4(float (&v)[8], const uint4 u) {   // v += u (8 halves)
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    for (int h = 0; h < 2; ++h) map_row(p, m_tile, r_local + 8 * h, &out_row[h], &sample[h]);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 a = unpack_h2(w[j]);
-    v[2 * j] += a.x;
-    v[2 * j + 1] += a.y;
-  }
-}
-__device__ __forceinline__ void round_add_u4(float (&v)[8], const uint4 u) {   // v = fp16(v) + u (8 halves)
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    for (int i = 0; i < BN / 8; ++i) {
+      const bool ok = n0 + i * 8 < p.N;
+      bias[i] = (p.bias && ok) ? __ldg(reinterpret_cast<const uint32_t*>(p.bias + n0 + i * 8 + 2 * q)) : 0u;
+      if (SC) bias_sc[i] = (p.bias_sc && ok) ? __ldg(reinterpret_cast<const uint32_t*>(p.bias_sc + n0 + i * 8 + 2 * q)) : 0u;
+    }
+    if (HAS_RES) {
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 a = unpack_h2(w[j]);
-    v[2 * j] = round_h(v[2 * j]) + a.x;
-    v[2 * j + 1] = round_h(v[2 * j + 1]) + a.y;
+      for (int c = 0; c < RES_AHEAD; ++c) load_res(p, c);
+    }
   }
-}
-__device__ __forceinline__ void round_add_h8(float (&v)[8], const __half* src) {   // v = fp16(v) + src
-  const uint4 u = *reinterpret_cast<const uint4*>(src);
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 a = unpack_h2(w[j]);
-    v[2 * j] = round_h(v[2 * j]) + a.x;
-    v[2 * j + 1] = round_h(v[2 * j + 1]) + a.y;
-  }
-}
 
-// One 32-column chunk of the fused epilogue for one accumulator row: registers -> (bias, activation, temb, shortcut,
-// residual with the reference's fp16 rounding points) -> 16 packed half2 words. Columns >= N of the last tile carry
-// don't-care values (the sinks clip them).
-template <int BN, bool GEGLU, int EPI>
-__device__ __forceinline__ void epilogue_math(const GemmParams& p, int n_tile, long long out_row, int sample, int c,
-                                              const uint32_t (&acc)[32], const uint32_t (&acc2)[32], uint32_t (&pk)[16],
-                                              const uint4* res_pre = nullptr, const uint4* bias_pre = nullptr) {
-  constexpr bool RT = (EPI & EPI_RUNTIME) != 0;
-  const bool has_bias = RT ? (p.bias != nullptr) : ((EPI & EPI_BIAS) != 0);
-  const bool has_rowvec = RT ? (p.rowvec != nullptr) : ((EPI & EPI_ROWVEC) != 0);
-  const bool has_res = RT ? (p.residual != nullptr) : ((EPI & EPI_RES) != 0);
-  const int n0 = n_tile * BN;
-  const int out_n0 = GEGLU ? n_tile * (BN / 2) : n0;
-  const int out_N = GEGLU ? p.N / 2 : p.N;
-  // Rows outside the output (a conv box whose batch extent exceeds B, the ragged last M tile) carry a sample index past
-  // the [B, ld_rowvec] time-embedding tensor: their values are never stored, so they must not read it either (found by
-  // compute-sanitizer in round 2: a 16-byte read up to bb - B rows past the tensor).
-  const __half* rowvec_row = (has_rowvec && out_row >= 0) ? p.rowvec + static_cast<long long>(sample) * p.ld_rowvec : nullptr;
-  const __half* res_row = (has_res && out_row >= 0) ? p.residual + out_row * p.ld_res : nullptr;
+  __device__ __forceinline__ void finish(const GemmParams& p, const float (&acc)[BN / 2], const float (&acc_sc)[BN / 2]) {
+    // Rows outside the output (a conv box whose batch extent exceeds B, the ragged last M tile) carry a sample index past
+    // the [B, ld_rowvec] time-embedding tensor: their values are never stored, so they must not read it either.
+    const __half* rowvec_row[2];
 #pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const int ncol = out_n0 + c * 32 + g * 8;  // output column of this 8-group
-    const bool col_ok = ncol < out_N;
-    float v[8];
+    for (int h = 0; h < 2; ++h)
+      rowvec_row[h] = (p.rowvec && out_row[h] >= 0) ? p.rowvec + static_cast<long long>(sample[h]) * p.ld_rowvec : nullptr;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(acc[g * 8 + j]);
-    if (GEGLU) {
-      const int bcol = n0 + c * 32 + g * 8;  // packed (interleaved) bias index of the value half
-      float gt[8];
+    for (int c = 0; c < CHUNKS; ++c) {
+      if (out_n0 + c * 32 >= out_N) break;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) gt[j] = __uint_as_float(acc2[g * 8 + j]);
-      if (p.bias && col_ok) {
-        add_h8(v, p.bias + bcol);
-        add_h8(gt, p.bias + bcol + BN / 2);
-      }
+      for (int h = 0; h < 2; ++h) {
+        uint32_t w[4];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float hv = round_h(v[j]);
-        const float gv = round_h(gt[j]);
-        v[j] = hv * round_h(gelu_erf_fast(gv));  // fp16(h) * fp16(gelu(fp16(gate)))
-      }
-    } else {
-      if (bias_pre != nullptr) {
-        if (has_bias) add_u4(v, bias_pre[g]);   // prefetched by the caller (zeros past N)
-      } else if (has_bias && col_ok) {
-        add_h8(v, p.bias + ncol);
-      }
-      if (RT && p.act_gelu) {   // rare (Resampler FeedForward, CLIP MLPs): keep it rolled
-#pragma unroll 1
-        for (int j = 0; j < 8; ++j) {
-          const float x = round_h(v[j]);
-          // 1: erf-GELU; 2: quick-GELU x * sigmoid(1.702 x) (the CLIP ViT-L text encoder's activation)
-          v[j] = p.act_gelu == 2 ? __fdividef(x, 1.0f + __expf(-1.702f * x)) : gelu_erf_fast(x);
+        for (int g = 0; g < 4; ++g) {
+          const int i = 4 * c + g;
+          const bool col_ok = out_n0 + i * 8 < out_N;
+          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          if (GEGLU) {   // packed (interleaved) bias: value half at n0 + 8i, gate half BN/2 further
+            float g0 = acc[4 * (i + BN / 16) + 2 * h], g1 = acc[4 * (i + BN / 16) + 2 * h + 1];
+            if (p.bias && col_ok) {
+              const float2 b = unpack_h2(bias[i]), bg = unpack_h2(bias[i + BN / 16]);
+              v0 += b.x, v1 += b.y, g0 += bg.x, g1 += bg.y;
+            }
+            v0 = round_h(v0) * round_h(gelu_erf_fast(round_h(g0)));   // fp16(h) * fp16(gelu(fp16(gate)))
+            v1 = round_h(v1) * round_h(gelu_erf_fast(round_h(g1)));
+          } else {
+            if (p.bias && col_ok) {
+              const float2 b = unpack_h2(bias[i]);
+              v0 += b.x, v1 += b.y;
+            }
+            if (p.act_gelu) {   // rare (Resampler FeedForward, CLIP MLPs)
+              const float x0 = round_h(v0), x1 = round_h(v1);
+              // 1: erf-GELU; 2: quick-GELU x * sigmoid(1.702 x) (the CLIP ViT-L text encoder's activation)
+              v0 = p.act_gelu == 2 ? __fdividef(x0, 1.0f + __expf(-1.702f * x0)) : gelu_erf_fast(x0);
+              v1 = p.act_gelu == 2 ? __fdividef(x1, 1.0f + __expf(-1.702f * x1)) : gelu_erf_fast(x1);
+            }
+            if (rowvec_row[h] != nullptr && col_ok) {
+              const float2 t = ldg_h2(rowvec_row[h] + n0 + i * 8 + 2 * q);
+              v0 = round_h(v0) + t.x, v1 = round_h(v1) + t.y;
+            }
+            if (SC) {
+              float s0 = acc_sc[4 * i + 2 * h], s1 = acc_sc[4 * i + 2 * h + 1];
+              if (p.bias_sc && col_ok) {
+                const float2 b = unpack_h2(bias_sc[i]);
+                s0 += b.x, s1 += b.y;
+              }
+              v0 = round_h(s0) + round_h(v0), v1 = round_h(s1) + round_h(v1);
+            }
+          }
+          w[g] = pack_h2(v0, v1);
         }
-      }
-      if (has_rowvec && col_ok && rowvec_row != nullptr) round_add_h8(v, rowvec_row + ncol);
-      if (RT && p.slabs_sc) {
-        float s[8];
+        quad_transpose(w, q);
+        if (out_row[h] < 0 || own_col(c) >= out_N) continue;
+        if (HAS_RES && p.residual) {
+          const uint4 u = res[h][c % RES_AHEAD];
+          const uint32_t r[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
-        for (int j = 0; j < 8; ++j) s[j] = __uint_as_float(acc2[g * 8 + j]);
-        if (p.bias_sc && col_ok) add_h8(s, p.bias_sc + ncol);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = round_h(s[j]) + round_h(v[j]);
+          for (int j = 0; j < 4; ++j) {   // w already holds fp16(v)
+            const float2 a = unpack_h2(w[j]), d = unpack_h2(r[j]);
+            w[j] = pack_h2(a.x + d.x, a.y + d.y);
+          }
+        }
+        *reinterpret_cast<uint4*>(p.out + out_row[h] * p.ld_out + own_col(c)) = make_uint4(w[0], w[1], w[2], w[3]);
       }
-      if (res_pre != nullptr) {   // residual row segment prefetched by the caller (zeros where it does not apply)
-        if (has_res) round_add_u4(v, res_pre[g]);
-      } else if (has_res && col_ok && res_row != nullptr) {
-        round_add_h8(v, res_row + ncol);
-      }
-    }
-    pk[g * 4 + 0] = pack_h2(v[0], v[1]);
-    pk[g * 4 + 1] = pack_h2(v[2], v[3]);
-    pk[g * 4 + 2] = pack_h2(v[4], v[5]);
-    pk[g * 4 + 3] = pack_h2(v[6], v[7]);
-  }
-}
-
-// Registers -> global, each thread writes the 32-column chunks c = c_first, c_first + c_step, ... of its own row.
-template <int BN, bool GEGLU>
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float* row, const float* row_sc, int n_tile,
-                                               long long out_row, int sample, int c_first, int c_step) {
-  constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
-  const int out_n0 = GEGLU ? n_tile * (BN / 2) : n_tile * BN;
-  const int out_N = GEGLU ? p.N / 2 : p.N;
-#pragma unroll 1
-  for (int c = c_first; c < OUT_COLS / 32; c += c_step) {
-    if (out_row < 0 || out_n0 + c * 32 >= out_N) continue;
-    uint32_t acc[32], acc2[32];
-    uint32_t pk[16];
-    epilogue_load<BN, GEGLU, EPI_RUNTIME>(p, row, row_sc, c, acc, acc2);
-    epilogue_math<BN, GEGLU, EPI_RUNTIME>(p, n_tile, out_row, sample, c, acc, acc2, pk);
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int ncol = out_n0 + c * 32 + g * 8;
-      if (ncol >= out_N) continue;
-      *reinterpret_cast<uint4*>(p.out + out_row * p.ld_out + ncol) =
-          make_uint4(pk[g * 4], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
+      if (HAS_RES && c + RES_AHEAD < CHUNKS) load_res(p, c + RES_AHEAD);
     }
   }
-}
+};
 
-// ----------------------------------------------------------------------------------------------
-// TMA stores (smem -> global, bulk async group); out-of-bounds box elements are clipped by the hardware.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_all() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+// fp32-output epilogue (the VAE convolutions) from the same fragment: out = acc + bias (+ residual), all fp32. A thread
+// stores float2 pairs, a quad one 32-byte sector per row.
+template <int BN>
+__device__ __forceinline__ void epilogue_f32(const GemmParams& p, int m_tile, int n_tile, int r_local,
+                                             const float (&acc)[BN / 2]) {
+  const int q = threadIdx.x & 3;
+  const int n0 = n_tile * BN;
+  long long out_row[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int sample;
+    map_row(p, m_tile, r_local + 8 * h, &out_row[h], &sample);
+  }
+#pragma unroll
+  for (int i = 0; i < BN / 8; ++i) {
+    if (n0 + i * 8 >= p.N) break;
+    const int ncol = n0 + i * 8 + 2 * q;
+    float2 b = make_float2(0.0f, 0.0f);
+    if (p.bias_f32 != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias_f32 + ncol));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (out_row[h] < 0) continue;
+      float2 v = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      if (p.bias_f32 != nullptr) v.x += b.x, v.y += b.y;
+      if (p.res_f32 != nullptr) {   // after the bias, like torch's `x + conv(h)`
+        const float2 r = __ldg(reinterpret_cast<const float2*>(p.res_f32 + out_row[h] * p.N + ncol));
+        v.x += r.x, v.y += r.y;
+      }
+      *reinterpret_cast<float2*>(p.out_f32 + out_row[h] * p.N + ncol) = v;
+    }
+  }
 }
 
 }  // namespace vton
