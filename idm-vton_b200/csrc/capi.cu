@@ -7,6 +7,11 @@ namespace vton {
 int gemm_f16_impl(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldo, int M, int N,
                   int K, const void* bias, const void* residual, long long ldr, const void* rowvec, long long ld_rowvec,
                   int rows_per_sample, int flags, int force_bn, cudaStream_t stream);
+int gemm_e4m3_impl(const void* A, long long lda, const void* a_scale, const void* W, long long ldw, const void* w_scale,
+                   void* out, long long ldo, int M, int N, int K, const void* bias, const void* residual, long long ldr,
+                   int flags, int force_bn, cudaStream_t stream);
+int layernorm_e4m3_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
+                        void* out, long long ldo, void* q, long long ldq, void* q_scale, cudaStream_t stream);
 int conv3x3_impl(const void* x, long long ldx, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
                  const void* temb, long long ld_temb, const void* sc0, int C0, const void* sc1, int C1, const void* w_sc,
                  const void* bias_sc, const void* residual, long long ldr, void* out, long long ldo, int force_bn,
@@ -107,6 +112,13 @@ int b200vton_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, vo
                              rows_per_sample, flags, force_bn, S(stream));
 }
 
+int b200vton_gemm_e4m3(const void* A_q, int64_t lda, const void* a_scale, const void* W_q, int64_t ldw,
+                       const void* w_scale, void* out, int64_t ldo, int M, int N, int K, const void* bias,
+                       const void* residual, int64_t ldr, int flags, int force_bn, void* stream) {
+  return vton::gemm_e4m3_impl(A_q, lda, a_scale, W_q, ldw, w_scale, out, ldo, M, N, K, bias, residual, ldr, flags,
+                              force_bn, S(stream));
+}
+
 int b200vton_conv3x3_nhwc(const void* x, int64_t ldx, int B, int H, int W, int Cin, const void* w, int Cout,
                           const void* bias, const void* temb, int64_t ld_temb, const void* sc0, int C0,
                           const void* sc1, int C1, const void* w_sc, const void* bias_sc, const void* residual,
@@ -171,6 +183,11 @@ int b200vton_groupnorm(const void* x0, int C0, const void* x1, int C1, int B, in
 int b200vton_layernorm(const void* x, int64_t ldx, int rows, int C, const void* gamma, const void* beta, float eps,
                        void* out, int64_t ldo, void* stream) {
   return vton::layernorm_impl(x, ldx, rows, C, gamma, beta, eps, out, ldo, S(stream));
+}
+
+int b200vton_layernorm_e4m3(const void* x, int64_t ldx, int rows, int C, const void* gamma, const void* beta,
+                            float eps, void* out, int64_t ldo, void* q, int64_t ldq, void* q_scale, void* stream) {
+  return vton::layernorm_e4m3_impl(x, ldx, rows, C, gamma, beta, eps, out, ldo, q, ldq, q_scale, S(stream));
 }
 
 int b200vton_nchw_to_nhwc(const void* src, int Bs, int Cs, int H, int W, void* dst, int Bd, int ldc, int c_off,

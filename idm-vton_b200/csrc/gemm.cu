@@ -14,6 +14,13 @@
 // epilogue on its own accumulator fragment (gemm_common.cuh) and stores 16 bytes at a time. The epilogue does not touch
 // shared memory, so the producer runs on into the next tile's slabs meanwhile and the operand ring is full again when
 // the consumers come back: only a CTA's first tile waits for a load.
+// e4m3 linears (KIND_E4M3, the opt-in FP8 mode): a 128-byte slab row holds 128 e4m3 values, so the ring, the
+// descriptors and the 32-byte MMA step are those of the fp16 kind; the MMA is m64nNk32 e4m3 x e4m3 -> fp32 and the
+// epilogue scales each accumulator by its row's and column's scale before the fp16 epilogue below. The tensor core
+// keeps fewer accumulator bits for e4m3 than fp32 (the error grew with K to 4.5e-3 of the output's scale at K = 5120 on
+// an H100), so each slab's 4 MMAs accumulate into a partial sum of their own, which is added to the fp32 register
+// accumulator once the slab's MMAs have retired (E4M3_SUB columns at a time: halves at BN = 192 and quarters at BN = 256,
+// where a wider partial sum would not fit beside the accumulator without spilling).
 // Epilogue rounding points replicate the reference's fp16-autocast path (SURVEY.md App. D.1):
 //   v = fp16(acc + bias); v = fp16(v + temb[b,n]); s = fp16(acc_sc + bias_sc); v = fp16(s + v); v = fp16(v + res)
 #include "gemm_common.cuh"
@@ -22,11 +29,11 @@
 
 namespace vton {
 
-enum : int { KIND_F16 = 0, KIND_F16IN_F32OUT = 1, KIND_TF32 = 2 };
+enum : int { KIND_F16 = 0, KIND_F16IN_F32OUT = 1, KIND_TF32 = 2, KIND_E4M3 = 3 };
 
 template <int BN, int STAGES>
 struct SmemLayout {
-  static constexpr int B_BYTES = BN * 128;              // BN rows x 128 B (64 halves or 32 floats)
+  static constexpr int B_BYTES = BN * 128;              // BN rows x 128 B (64 halves, 32 floats or 128 e4m3)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;   // the barriers follow the operand ring
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;     // barriers + alignment slack
@@ -39,13 +46,17 @@ constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_PRODUCER_REGS = 40;
 constexpr int GEMM_CONSUMER_REGS = 232;
 
+template <int BN>
+constexpr int E4M3_SUB = BN == 256 ? 64 : (BN == 192 ? 96 : BN);
+
 template <int BN, int STAGES, bool GEGLU, bool SC, int KIND>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmS0, const __grid_constant__ CUtensorMap tmS1,
                  const __grid_constant__ CUtensorMap tmBs, const GemmParams p) {
   using L = SmemLayout<BN, STAGES>;
-  constexpr int KBK = KIND == KIND_TF32 ? 32 : 64;   // channels per 128-byte slab row
+  constexpr int KBK = KIND == KIND_TF32 ? 32 : (KIND == KIND_E4M3 ? 128 : 64);   // channels per 128-byte slab row
+  constexpr bool F16_EPI = KIND == KIND_F16 || KIND == KIND_E4M3;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
@@ -160,16 +171,48 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (s > 0) release(it - 1);   // s == 0: the previous slab was the last of the tile before and is released already
     }
   };
+  // e4m3: every slab accumulates into `part` (scale_d = 0 on its first MMA; 32 e4m3 = 32 bytes per MMA step), then
+  // acc += part after wait<0>; the slab is released right there, as all of its MMAs have retired.
+  auto run_slabs_promoted = [&](float (&accr)[BN / 2], int s_begin, int s_end) {
+    constexpr int SUB = E4M3_SUB<BN>;
+    for (int s = s_begin; s < s_end; ++s, ++it) {
+      const int stage = it % STAGES;
+      mbar_wait(full_bar(stage), (it / STAGES) & 1);
+      const uint32_t a_src = smem_base + stage * L::STAGE_BYTES + wg * (64 * 128);
+      const uint32_t b_src = smem_base + stage * L::STAGE_BYTES + A_BYTES;
+#pragma unroll
+      for (int sub = 0; sub < BN / SUB; ++sub) {
+        float part[SUB / 2];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = make_gmma_desc_sw128(a_src + k * 32, 0, 1024);
+          const uint64_t db = make_gmma_desc_sw128(b_src + sub * SUB * 128 + k * 32, 0, 1024);
+          WgmmaE4M3SS<SUB>::mma(part, da, db, k > 0 ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(part);
+#pragma unroll
+        for (int j = 0; j < SUB / 2; ++j) accr[sub * (SUB / 2) + j] = s > s_begin ? accr[sub * (SUB / 2) + j] + part[j] : part[j];
+      }
+      release(it);
+    }
+  };
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    EpilogueF16<BN, GEGLU, SC> epi;   // fp16 kinds: the tile's bias and first residual loads fly during the K loop
-    if constexpr (KIND == KIND_F16) epi.begin(p, tile / p.n_tiles, tile % p.n_tiles, r_local);
-    run_slabs(acc, 0, p.slabs_main);
-    if constexpr (SC) run_slabs(acc_sc, p.slabs_main, total_slabs);
-    wgmma_wait<0>();
-    fence_regs(acc);
-    if (SC) fence_regs(acc_sc);
-    release(it - 1);
-    if constexpr (KIND == KIND_F16) {
+    EpilogueF16<BN, GEGLU, SC, KIND == KIND_E4M3> epi;   // fp16 output: bias / residual loads fly during the K loop
+    if constexpr (F16_EPI) epi.begin(p, tile / p.n_tiles, tile % p.n_tiles, r_local);
+    if constexpr (KIND == KIND_E4M3) {
+      run_slabs_promoted(acc, 0, p.slabs_main);
+    } else {
+      run_slabs(acc, 0, p.slabs_main);
+      if constexpr (SC) run_slabs(acc_sc, p.slabs_main, total_slabs);
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (SC) fence_regs(acc_sc);
+      release(it - 1);
+    }
+    if constexpr (F16_EPI) {
       epi.finish(p, acc, acc_sc);
     } else {
       epilogue_f32<BN>(p, tile / p.n_tiles, tile % p.n_tiles, r_local, acc);
@@ -237,29 +280,32 @@ static int pick_bn(int N, int m_tiles, bool geglu, bool has_shortcut, int force_
   return best_bn ? best_bn : 128;
 }
 
+template <int KIND>
 static int dispatch(int bn, bool geglu, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmS0,
                     const CUtensorMap& tmS1, const CUtensorMap& tmBs, GemmParams& p, int m_tiles,
                     cudaStream_t stream) {
   p.n_tiles = cdiv(p.N, bn);
   p.total_tiles = m_tiles * p.n_tiles;
   if (geglu) {
-    if (bn == 128) return launch_variant<128, 6, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    if (bn == 256) return launch_variant<256, 4, true, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    if (bn == 128) return launch_variant<128, 6, true, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    if (bn == 256) return launch_variant<256, 4, true, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
     set_last_error("GEGLU epilogue supports BN 128/256 only (got %d)", bn);
     return kErrUnsupported;
   }
-  if (p.slabs_sc) {
-    if (bn == 64) return launch_variant<64, 8, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    if (bn == 128) return launch_variant<128, 6, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    set_last_error("shortcut epilogue supports BN 64/128 only (got %d)", bn);
-    return kErrUnsupported;
+  if constexpr (KIND == KIND_F16) {   // the fused shortcut exists for the fp16 convolution only
+    if (p.slabs_sc) {
+      if (bn == 64) return launch_variant<64, 8, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+      if (bn == 128) return launch_variant<128, 6, false, true, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+      set_last_error("shortcut epilogue supports BN 64/128 only (got %d)", bn);
+      return kErrUnsupported;
+    }
   }
   switch (bn) {
-    case 64: return launch_variant<64, 8, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    case 128: return launch_variant<128, 6, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    case 160: return launch_variant<160, 5, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    case 192: return launch_variant<192, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    case 256: return launch_variant<256, 4, false, false, KIND_F16>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 64: return launch_variant<64, 8, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 128: return launch_variant<128, 6, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 160: return launch_variant<160, 5, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 192: return launch_variant<192, 4, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 256: return launch_variant<256, 4, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
   }
   set_last_error("unsupported BN %d", bn);
   return kErrUnsupported;
@@ -307,7 +353,56 @@ int gemm_f16_impl(const void* A, long long lda, const void* W, long long ldw, vo
   p.rows_per_sample = rows_per_sample;
   p.slabs_main = K / 64;
   p.act_gelu = (flags & 4) ? 2 : ((flags & 2) ? 1 : 0);
-  return dispatch(bn, geglu != 0, tmA, tmB, tmA, tmA, tmB, p, cdiv(M, BM), stream);
+  return dispatch<KIND_F16>(bn, geglu != 0, tmA, tmB, tmA, tmA, tmB, p, cdiv(M, BM), stream);
+}
+
+// A_q [M, lda] and W_q [N, ldw] e4m3 (lda / ldw in elements = bytes), a_scale [M] and w_scale [N] fp32: the per-row
+// (per-token) and per-output-channel scales of the FP8 linears. out = epi((acc * a_scale[m]) * w_scale[n]) with the fp16
+// epilogue of gemm_f16_impl (bias, GEGLU, residual); flags & 1 = GEGLU, no other flag.
+int gemm_e4m3_impl(const void* A, long long lda, const void* a_scale, const void* W, long long ldw, const void* w_scale,
+                   void* out, long long ldo, int M, int N, int K, const void* bias, const void* residual, long long ldr,
+                   int flags, int force_bn, cudaStream_t stream) {
+  const int geglu = flags & 1;
+  VTON_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm_e4m3: empty problem M=%d N=%d K=%d", M, N, K);
+  VTON_CHECK_ARG(K % 128 == 0, "gemm_e4m3: K=%d must be a multiple of 128", K);
+  VTON_CHECK_ARG((flags & ~1) == 0, "gemm_e4m3: flags=%d unsupported (only GEGLU = 1)", flags);
+  VTON_CHECK_ARG(A && W && out && a_scale && w_scale, "gemm_e4m3: A, W, out, a_scale and w_scale must not be null");
+  VTON_CHECK_ARG(lda % 16 == 0 && ldw % 16 == 0, "gemm_e4m3: lda=%lld / ldw=%lld must be multiples of 16 bytes", lda, ldw);
+  VTON_CHECK_ARG(N % 8 == 0 && ldo % 8 == 0, "gemm_e4m3: N/ldo must be multiples of 8");
+  VTON_CHECK_ARG(!geglu || (N % 16 == 0 && !residual), "gemm_e4m3: bad GEGLU configuration");
+  VTON_CHECK_ARG(aligned_to(A, 16) && aligned_to(W, 16) && aligned_to(out, 16) && aligned_to(bias, 16) &&
+                     aligned_to(residual, 16) && aligned_to(a_scale, 4) && aligned_to(w_scale, 8),
+                 "gemm_e4m3: A/W/out/bias/residual must be 16-byte aligned, a_scale 4-byte, w_scale 8-byte");
+  VTON_CHECK_ARG(!residual || ldr % 8 == 0, "gemm_e4m3: ldr=%lld must be a multiple of 8", ldr);
+  const int bn = pick_bn(N, cdiv(M, BM), geglu != 0, false, force_bn);
+  VTON_CHECK_ARG(bn != 0, "gemm_e4m3: tile width force_bn=%d unsupported for this problem (N=%d, geglu=%d)", force_bn, N,
+                 geglu);
+  VTON_CHECK_ARG(!geglu || N % bn == 0, "gemm_e4m3: GEGLU needs N %% BN == 0 (N=%d, BN=%d)", N, bn);
+  CUtensorMap tmA, tmB;
+  {
+    uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(M)};
+    uint64_t strides[1] = {static_cast<uint64_t>(lda)};
+    uint32_t box[2] = {128, 128};
+    if (int e = encode_tmap_u8(&tmA, A, 2, dims, strides, box)) return e;
+  }
+  {
+    uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
+    uint64_t strides[1] = {static_cast<uint64_t>(ldw)};
+    uint32_t box[2] = {128, static_cast<uint32_t>(bn)};
+    if (int e = encode_tmap_u8(&tmB, W, 2, dims, strides, box)) return e;
+  }
+  GemmParams p{};
+  p.out = static_cast<__half*>(out);
+  p.ld_out = static_cast<int>(ldo);
+  p.M = M;
+  p.N = N;
+  p.bias = static_cast<const __half*>(bias);
+  p.residual = static_cast<const __half*>(residual);
+  p.ld_res = static_cast<int>(ldr);
+  p.slabs_main = K / 128;
+  p.a_scale = static_cast<const float*>(a_scale);
+  p.w_scale = static_cast<const float*>(w_scale);
+  return dispatch<KIND_E4M3>(bn, geglu != 0, tmA, tmB, tmA, tmA, tmB, p, cdiv(M, BM), stream);
 }
 
 static void pick_box(int B, int H, int W, int* bw, int* bh, int* bb) {
@@ -411,7 +506,7 @@ int conv3x3_impl(const void* x, long long ldx, int B, int Hin, int Win, int Cin,
   p.cin_slabs = Cin / 64;
   p.cout = Cout;
   const int m_tiles = p.tiles_x * p.tiles_y * cdiv(B, bb);
-  return dispatch(bn, false, tmA, tmB, tmS0, tmS1, tmBs, p, m_tiles, stream);
+  return dispatch<KIND_F16>(bn, false, tmA, tmB, tmS0, tmS1, tmBs, p, m_tiles, stream);
 }
 
 // x: [B,H,W,Cin] fp32 NHWC (dense), w: [9][Cout][Cin] fp32 (tap-major), bias: [Cout] fp32 or null, residual: [B,H,W,Cout]

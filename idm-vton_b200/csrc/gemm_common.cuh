@@ -35,6 +35,9 @@ struct GemmParams {
   float* out_f32;
   const float* bias_f32;
   const float* res_f32;
+  // e4m3 operands (the FP8 linears): acc is scaled to (acc * a_scale[m]) * w_scale[n] before the fp16 epilogue
+  const float* a_scale;
+  const float* w_scale;
 };
 
 constexpr int BM = 128;
@@ -119,12 +122,16 @@ __device__ __forceinline__ float2 ldg_h2(const __half* src) {
 // before the tile's K loop: it maps the rows and issues the loads of the tile's bias words and of the first RES_AHEAD
 // chunks of the residual, which land while the tensor cores work. finish() runs after the K loop and keeps the residual
 // RES_AHEAD chunks ahead of the chunk it stores; a consumed chunk frees 16 accumulator registers for the 8 it loads.
-template <int BN, bool GEGLU, bool SC>
+// SCALED (e4m3 operands): every accumulator is first scaled to (acc * a_scale[row]) * w_scale[col] in fp32; the row
+// scales are loaded in begin(), the column scales of an 8-group where it is scaled (L1 hits after the first row; BN/4
+// more registers held across the K loop would not fit at BN = 256). Everything after that is the fp16 epilogue unchanged.
+template <int BN, bool GEGLU, bool SC, bool SCALED = false>
 struct EpilogueF16 {
   static constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
   static constexpr int CHUNKS = OUT_COLS / 32;
   static constexpr bool HAS_RES = !GEGLU && !SC;   // a residual comes with neither GEGLU nor a fused shortcut
-  static constexpr int RES_AHEAD = !HAS_RES ? 1 : (CHUNKS < 4 ? CHUNKS : 4);
+  // SCALED: the e4m3 main loop holds a partial-sum accumulator beside acc, so the residual is loaded one chunk ahead only
+  static constexpr int RES_AHEAD = (!HAS_RES || SCALED) ? 1 : (CHUNKS < 4 ? CHUNKS : 4);
 
   int q, n0, out_n0, out_N;
   long long out_row[2];
@@ -132,6 +139,7 @@ struct EpilogueF16 {
   uint32_t bias[BN / 8];              // half2 of columns n0 + 8i + 2q + {0,1} (GEGLU: value and gate halves alike)
   uint32_t bias_sc[SC ? BN / 8 : 1];
   uint4 res[2][RES_AHEAD];            // residual of chunk c in slot c % RES_AHEAD, in the transposed (stored) shape
+  float a_scale[SCALED ? 2 : 1];      // row scales of rows r_local and r_local + 8
 
   __device__ __forceinline__ int own_col(int c) const { return out_n0 + (4 * c + q) * 8; }   // this lane's 8-group of chunk c
 
@@ -152,6 +160,10 @@ struct EpilogueF16 {
     out_N = GEGLU ? p.N / 2 : p.N;
 #pragma unroll
     for (int h = 0; h < 2; ++h) map_row(p, m_tile, r_local + 8 * h, &out_row[h], &sample[h]);
+    if constexpr (SCALED) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) a_scale[h] = out_row[h] >= 0 ? __ldg(p.a_scale + out_row[h]) : 0.0f;
+    }
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
       const bool ok = n0 + i * 8 < p.N;
@@ -182,8 +194,23 @@ struct EpilogueF16 {
           const int i = 4 * c + g;
           const bool col_ok = out_n0 + i * 8 < out_N;
           float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          float2 w_scale[GEGLU ? 2 : 1];   // column scales of the 8-group (GEGLU: and of its gate columns)
+          if constexpr (SCALED) {
+#pragma unroll
+            for (int e = 0; e < (GEGLU ? 2 : 1); ++e) {
+              const int col = n0 + (i + e * (BN / 16)) * 8 + 2 * q;
+              w_scale[e] = col < p.N ? __ldg(reinterpret_cast<const float2*>(p.w_scale + col)) : make_float2(0.f, 0.f);
+            }
+            // __fmul_rn: the scaled product is rounded to fp32 before the bias add (no FMA contraction)
+            v0 = __fmul_rn(__fmul_rn(v0, a_scale[h]), w_scale[0].x);
+            v1 = __fmul_rn(__fmul_rn(v1, a_scale[h]), w_scale[0].y);
+          }
           if (GEGLU) {   // packed (interleaved) bias: value half at n0 + 8i, gate half BN/2 further
             float g0 = acc[4 * (i + BN / 16) + 2 * h], g1 = acc[4 * (i + BN / 16) + 2 * h + 1];
+            if constexpr (SCALED) {
+              g0 = __fmul_rn(__fmul_rn(g0, a_scale[h]), w_scale[GEGLU ? 1 : 0].x);
+              g1 = __fmul_rn(__fmul_rn(g1, a_scale[h]), w_scale[GEGLU ? 1 : 0].y);
+            }
             if (p.bias && col_ok) {
               const float2 b = unpack_h2(bias[i]), bg = unpack_h2(bias[i + BN / 16]);
               v0 += b.x, v1 += b.y, g0 += bg.x, g1 += bg.y;

@@ -107,4 +107,9 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
   return encode_tmap_any(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box, nullptr, 128);
 }
 
+int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                   const uint32_t* box) {
+  return encode_tmap_any(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, nullptr, 128);
+}
+
 }  // namespace vton

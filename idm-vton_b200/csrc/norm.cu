@@ -8,6 +8,8 @@
 //              The input may be the channel-concat of two tensors (up-block skip, src/unet_block_hacked_tryon.py:2346)
 //              which is never materialised: both sources are read in place.
 //   LayerNorm: BasicTransformerBlock.norm1/2/3 (src/attentionhacked_tryon.py:310,365,390), eps 1e-5.
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 #include "host.h"
 
@@ -338,10 +340,13 @@ constexpr int LN_MAX_VEC = 8;  // per lane: up to 8 x 8 halves => C <= 2048
 
 // NV = ceil(C / 256) uint4 loads per lane, a compile-time bound so the row lives in 8*NV registers (C = 640: 24,
 // C = 1280: 40) and the SM holds enough warps to cover the load latency.
-template <int NV>
+// QUANT (layernorm_e4m3, the FP8 linears' input): the same arithmetic gives the fp16 row y16; then amax = max|y16|
+// over the row, scale = amax / 448 and q = e4m3_rn_satfinite(y16 * (448 / amax)) (an all-zero row: scale 1, q 0).
+// `out` (the fp16 row, bit-identical to the plain LayerNorm) is optional then.
+template <int NV, bool QUANT>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const __half* x, long long ldx, int rows, int C, const __half* gamma, const __half* beta, float eps,
-                 __half* out, long long ldo) {
+                 __half* out, long long ldo, __nv_fp8_storage_t* q, long long ldq, float* q_scale) {
   pdl_launch_dependents();
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -383,6 +388,8 @@ layernorm_kernel(const __half* x, long long ldx, int rows, int C, const __half* 
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
   const float rstd = rsqrtf(sq / C + eps);
+  uint32_t yw[QUANT ? NV : 1][4];   // the fp16 row, kept for the quantization pass
+  float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int v = lane + i * 32;
@@ -399,10 +406,63 @@ layernorm_kernel(const __half* x, long long ldx, int rows, int C, const __half* 
         const float y0 = (val[i][2 * j] - mean) * rstd * gg.x + bb.x;
         const float y1 = (val[i][2 * j + 1] - mean) * rstd * gg.y + bb.y;
         ow[j] = pack_h2(y0, y1);
+        if constexpr (QUANT) {
+          const float2 y = unpack_h2(ow[j]);
+          amax = fmaxf(amax, fmaxf(fabsf(y.x), fabsf(y.y)));
+          yw[i][j] = ow[j];
+        }
       }
-      *reinterpret_cast<uint4*>(out + row * ldo + v * 8) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      if (!QUANT || out != nullptr)
+        *reinterpret_cast<uint4*>(out + row * ldo + v * 8) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
     }
   }
+  if constexpr (QUANT) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float inv = amax > 0.f ? __fdiv_rn(448.0f, amax) : 0.f;
+    if (lane == 0) q_scale[row] = amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int v = lane + i * 32;
+      if (v < V) {
+        uint32_t qw[2];
+#pragma unroll
+        for (int j = 0; j < 4; j += 2) {
+          const float2 a = unpack_h2(yw[i][j]), b = unpack_h2(yw[i][j + 1]);
+          const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(a.x, inv), __fmul_rn(a.y, inv)),
+                                                                   __NV_SATFINITE, __NV_E4M3);
+          const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(b.x, inv), __fmul_rn(b.y, inv)),
+                                                                   __NV_SATFINITE, __NV_E4M3);
+          qw[j / 2] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+        }
+        *reinterpret_cast<uint2*>(q + row * ldq + v * 8) = make_uint2(qw[0], qw[1]);
+      }
+    }
+  }
+}
+
+template <bool QUANT>
+static int layernorm_launch(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
+                            void* out, long long ldo, void* q, long long ldq, void* q_scale, cudaStream_t stream) {
+  const int nv = cdiv(C / 8, 32);
+  auto go = [&](auto kern) {
+    return launch_kernel(kern, dim3(cdiv(rows, 8)), dim3(256), 0, stream, static_cast<const __half*>(x), ldx, rows, C,
+                         static_cast<const __half*>(gamma), static_cast<const __half*>(beta), eps,
+                         static_cast<__half*>(out), ldo, static_cast<__nv_fp8_storage_t*>(q), ldq,
+                         static_cast<float*>(q_scale));
+  };
+  cudaError_t le = cudaSuccess;
+  switch (nv) {
+    case 1: le = go(layernorm_kernel<1, QUANT>); break;
+    case 2: le = go(layernorm_kernel<2, QUANT>); break;
+    case 3: le = go(layernorm_kernel<3, QUANT>); break;
+    case 4: le = go(layernorm_kernel<4, QUANT>); break;
+    case 5: le = go(layernorm_kernel<5, QUANT>); break;
+    default: le = go(layernorm_kernel<LN_MAX_VEC, QUANT>); break;
+  }
+  VTON_CUDA(le);
+  count_launch();
+  return kOk;
 }
 
 int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
@@ -411,24 +471,20 @@ int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* ga
   VTON_CHECK_ARG(C % 8 == 0 && C <= LN_MAX_VEC * 256 && ldx % 8 == 0 && ldo % 8 == 0, "layernorm: C=%d unsupported", C);
   VTON_CHECK_ARG(aligned_to(x, 16) && aligned_to(out, 16) && aligned_to(gamma, 16) && aligned_to(beta, 16),
                  "layernorm: x/out/gamma/beta must be 16-byte aligned (read and written 8 halves at a time)");
-  const int nv = cdiv(C / 8, 32);
-  auto go = [&](auto kern) {
-    return launch_kernel(kern, dim3(cdiv(rows, 8)), dim3(256), 0, stream, static_cast<const __half*>(x), ldx, rows, C,
-                         static_cast<const __half*>(gamma), static_cast<const __half*>(beta), eps,
-                         static_cast<__half*>(out), ldo);
-  };
-  cudaError_t le = cudaSuccess;
-  switch (nv) {
-    case 1: le = go(layernorm_kernel<1>); break;
-    case 2: le = go(layernorm_kernel<2>); break;
-    case 3: le = go(layernorm_kernel<3>); break;
-    case 4: le = go(layernorm_kernel<4>); break;
-    case 5: le = go(layernorm_kernel<5>); break;
-    default: le = go(layernorm_kernel<LN_MAX_VEC>); break;
-  }
-  VTON_CUDA(le);
-  count_launch();
-  return kOk;
+  return layernorm_launch<false>(x, ldx, rows, C, gamma, beta, eps, out, ldo, nullptr, 0, nullptr, stream);
+}
+
+int layernorm_e4m3_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
+                        void* out, long long ldo, void* q, long long ldq, void* q_scale, cudaStream_t stream) {
+  VTON_CHECK_ARG(rows > 0 && C > 0, "layernorm_e4m3: empty input");
+  VTON_CHECK_ARG(C % 8 == 0 && C <= LN_MAX_VEC * 256 && ldx % 8 == 0 && (!out || ldo % 8 == 0),
+                 "layernorm_e4m3: C=%d unsupported", C);
+  VTON_CHECK_ARG(q && q_scale, "layernorm_e4m3: q and q_scale must not be null");
+  VTON_CHECK_ARG(ldq % 16 == 0 && ldq >= C, "layernorm_e4m3: ldq=%lld must be a multiple of 16 and >= C", ldq);
+  VTON_CHECK_ARG(aligned_to(x, 16) && aligned_to(out, 16) && aligned_to(gamma, 16) && aligned_to(beta, 16) &&
+                     aligned_to(q, 16) && aligned_to(q_scale, 4),
+                 "layernorm_e4m3: x/out/q/gamma/beta must be 16-byte aligned, q_scale 4-byte");
+  return layernorm_launch<true>(x, ldx, rows, C, gamma, beta, eps, out, ldo, q, ldq, q_scale, stream);
 }
 
 }  // namespace vton

@@ -234,6 +234,11 @@ class GarmentKVCache:
         self.entries[key] = (tensors, n)
         self.bytes += n
 
+    def clear(self):
+        """Drops every entry (the pipeline's UNet arithmetic changed: cached K/V would no longer be what it computes)."""
+        self.entries.clear()
+        self.bytes = 0
+
 
 class TryOnDenoiser:
     def __init__(self, tryon: UNetEngine, garment: UNetEngine, hoist_garment=True, garment_chunk=None, max_kv_bytes=None):

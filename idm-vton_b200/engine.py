@@ -74,7 +74,7 @@ class _Resnet:
 
 class _Block:
     __slots__ = ("ln1w", "ln1b", "wqkv", "wo1", "bo1", "ln2w", "ln2b", "wq2", "wkv_txt", "wkv_ip", "wo2", "bo2", "ln3w",
-                 "ln3b", "wff1", "bff1", "wff2", "bff2", "c", "heads", "ff_bn", "ip_scale")
+                 "ln3b", "wff1", "bff1", "wff2", "bff2", "c", "heads", "ff_bn", "ip_scale", "fp8")
 
 
 class _T2D:
@@ -92,9 +92,12 @@ class UNetEngine:
 
     GEGLU_BN = 256
 
-    def __init__(self, cfg, state_dict, kind, device="cuda", ip_scales=None):
+    def __init__(self, cfg, state_dict, kind, device="cuda", ip_scales=None, fp8=False):
         """ip_scales: optional {"<transformer block path>": scale} of the installed IPAttnProcessor2_0 instances
-        (ip_adapter/attention_processor.py:1995 `hidden + self.scale * ip_hidden`; default 1.0)."""
+        (ip_adapter/attention_processor.py:1995 `hidden + self.scale * ip_hidden`; default 1.0).
+        fp8: run attn1's QKV, attn2.to_q and the GEGLU projection of every BasicTransformerBlock as e4m3 GEMMs, their
+        input quantized per token by the LayerNorm before them and the weights per output channel (INTEGRATION.md,
+        "FP8 linears"). Every channel width with a transformer must then be a multiple of 128."""
         from . import lib
         lib.load()
         self.L = lib
@@ -106,6 +109,12 @@ class UNetEngine:
         self.cross = cfg["cross_attention_dim"]
         self.ip_tokens = cfg["ip_tokens"] if kind == "tryon" else 0
         self.ip_scales = dict(ip_scales or {})
+        self.fp8 = bool(fp8)
+        if self.fp8:
+            for name in ("b200vton_layernorm_e4m3", "b200vton_gemm_e4m3"):
+                if not lib.has_symbol(name):
+                    raise NotImplementedError(f"FP8 linears need {name}, which {lib.LIB_PATH} does not export: rebuild it "
+                                              "(python idm-vton_b200/build.py --force)")
         self._pack(state_dict)
 
     # -------------------------------------------------------------------------------------------
@@ -161,8 +170,19 @@ class UNetEngine:
             blk.wff1, blk.bff1 = pack_geglu(self._w(sd, f"{b}.ff.net.0.proj.weight"),
                                             self._w(sd, f"{b}.ff.net.0.proj.bias"), bn)
             blk.wff2, blk.bff2 = self._w(sd, f"{b}.ff.net.2.weight"), self._w(sd, f"{b}.ff.net.2.bias")
+            blk.fp8 = self._pack_fp8(blk, b) if self.fp8 else None
             t.blocks.append(blk)
         return t
+
+    def _pack_fp8(self, blk, path):
+        """e4m3 weights and per-output-channel scales of the block's FP8 linears: {name: (w_q, w_scale)}. FF1 is quantized
+        after pack_geglu, so every interleaved row carries its own scale. FF2 stays fp16: its input (the GEGLU output)
+        would need a quantize pass of its own (BASELINE.md, "FP8 linears")."""
+        if blk.c % 128:
+            raise ValueError(f"{path}: FP8 linears need the channel width to be a multiple of 128 (got {blk.c}); there is "
+                             "no fp16 fallback in FP8 mode")
+        q = self.L.quantize_rows_e4m3
+        return dict(qkv=q(blk.wqkv), q2=q(blk.wq2), ff1=q(blk.wff1))
 
     def _pack(self, sd):
         cfg, ch = self.cfg, self.ch
@@ -304,14 +324,22 @@ class UNetEngine:
         n_garments, step_base int32 device scalar): garment K/V precomputed for all denoise steps."""
         L = self.L
         C, H = blk.c, blk.heads
-        n1 = L.layernorm(h, blk.ln1w, blk.ln1b)
+        f8 = blk.fp8
+        if f8 is not None:
+            # FP8 linears: each LayerNorm also writes its output quantized per row, the input of the e4m3 GEMM after it
+            n1q, n1s, n1 = L.layernorm_e4m3(h, blk.ln1w, blk.ln1b, fp16_out=collect is not None)
+        else:
+            n1 = L.layernorm(h, blk.ln1w, blk.ln1b)
         if collect is not None:
             collect.append(n1.view(B, N, C))                 # src/attentionhacked_garmnet.py:321-322
             if len(collect) == self.n_blocks:
                 # Last export of the garment UNet: everything after this norm1 (attn1/attn2/FF of this block, proj_out,
                 # the upsampler) only feeds `sample`, which the pipeline discards (src/tryon_pipeline.py:1787).
                 raise _GarmentDone()
-        qkv = L.gemm(n1, blk.wqkv).view(B, N, 3 * C)
+        if f8 is not None:
+            qkv = L.gemm_e4m3(n1q, n1s, *f8["qkv"]).view(B, N, 3 * C)
+        else:
+            qkv = L.gemm(n1, blk.wqkv).view(B, N, 3 * C)
         q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
         if gkv_pre is not None:
             kv_all, n_g, base = gkv_pre
@@ -325,8 +353,11 @@ class UNetEngine:
             off = 0 if bg == B else n_persons       # full-format features: every sample has its own segment 1
             a = L.attention(q, k, v, gkv[..., :C], gkv[..., C:], kv1_off=off, heads=H)
         h = L.gemm(a.view(B * N, C), blk.wo1, bias=blk.bo1, residual=h)
-        n2 = L.layernorm(h, blk.ln2w, blk.ln2b)
-        q2 = L.gemm(n2, blk.wq2).view(B, N, C)
+        if f8 is not None:
+            n2q, n2s, _ = L.layernorm_e4m3(h, blk.ln2w, blk.ln2b)
+            q2 = L.gemm_e4m3(n2q, n2s, *f8["q2"]).view(B, N, C)
+        else:
+            q2 = L.gemm(L.layernorm(h, blk.ln2w, blk.ln2b), blk.wq2).view(B, N, C)
         kv_t, kv_i = ctx
         if kv_t.shape[1] <= 80 and (kv_i is None or kv_i.shape[1] <= 16):
             # text + image-token cross-attention fused in one launch (both key sets fit one score tile)
@@ -338,9 +369,12 @@ class UNetEngine:
                 assert blk.ip_scale == 1.0, "ip scale != 1 needs the fused cross-attention kernel"
                 L.attention(q2, kv_i[..., :C], kv_i[..., C:], heads=H, accumulate=True, out=a2)
         h = L.gemm(a2.view(B * N, C), blk.wo2, bias=blk.bo2, residual=h)
-        n3 = L.layernorm(h, blk.ln3w, blk.ln3b)
-        ff = L.gemm(n3, blk.wff1, bias=blk.bff1, geglu=True,
-                    force_bn=blk.ff_bn)   # the tile width the GEGLU weights were packed for
+        # force_bn: the tile width the GEGLU weights were packed for
+        if f8 is not None:
+            n3q, n3s, _ = L.layernorm_e4m3(h, blk.ln3w, blk.ln3b)
+            ff = L.gemm_e4m3(n3q, n3s, *f8["ff1"], bias=blk.bff1, geglu=True, force_bn=blk.ff_bn)
+        else:
+            ff = L.gemm(L.layernorm(h, blk.ln3w, blk.ln3b), blk.wff1, bias=blk.bff1, geglu=True, force_bn=blk.ff_bn)
         return L.gemm(ff, blk.wff2, bias=blk.bff2, residual=h)
 
     def _t2d(self, t, x, state):

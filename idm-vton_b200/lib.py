@@ -48,11 +48,13 @@ SIGNATURES = {
 }
 
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
-# step kernels of the continuous-batching denoiser. `has_symbol` tells whether a binding can use them.
+# step kernels of the continuous-batching denoiser and the FP8 linears. `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
     "b200vton_cfg_solver_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "b200vton_nchw_to_nhwc_scaled_rows": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp],
+    "b200vton_gemm_e4m3": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _i64, _i, _i, _vp],
+    "b200vton_layernorm_e4m3": [_vp, _i64, _i, _i, _vp, _vp, _f, _vp, _i64, _vp, _i64, _vp, _vp],
 }
 _present = set()
 
@@ -447,6 +449,66 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     rc = lib.b200vton_layernorm(_p(x2), x2.stride(0), x2.shape[0], C, _p(gamma), _p(beta), float(eps), _p(o2),
                                 o2.stride(0), _stream())
     _check(rc, "b200vton_layernorm")
+    return out
+
+
+E4M3 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
+
+
+def layernorm_e4m3(x, gamma, beta, eps=1e-5, fp16_out=False):
+    """LayerNorm whose output feeds an FP8 linear: returns (q [rows, C] e4m3, scale [rows] fp32, y16 or None), with y16
+    the fp16 LayerNorm row (bit-identical to `layernorm`, written only when fp16_out), scale = max|y16| / 448 and
+    q = e4m3(y16 * 448 / max|y16|) (include/b200vton.h)."""
+    fn = _optional("b200vton_layernorm_e4m3")
+    _f16(x, "x")
+    C = x.shape[-1]
+    x2 = x.reshape(-1, C)
+    assert x2.stride(1) == 1
+    rows = x2.shape[0]
+    q = torch.empty((rows, C), dtype=E4M3, device=x.device)
+    scale = torch.empty(rows, dtype=torch.float32, device=x.device)
+    out = torch.empty((rows, C), dtype=torch.float16, device=x.device) if fp16_out else None
+    rc = fn(_p(x2), x2.stride(0), rows, C, _p(gamma), _p(beta), float(eps), _p(out), C if fp16_out else 0, _p(q),
+            q.stride(0), _p(scale), _stream())
+    _check(rc, "b200vton_layernorm_e4m3")
+    return q, scale, out
+
+
+def quantize_rows_e4m3(w):
+    """Per-row e4m3 quantization of an fp16 matrix with torch (the FP8 linears' weights, once at pack time): the rule of
+    layernorm_e4m3 applied to every row. Returns (q [N, K] e4m3, scale [N] fp32)."""
+    w32 = w.to(torch.float32)
+    amax = w32.abs().amax(dim=1)
+    nz = amax > 0
+    # tensor / tensor keeps IEEE division (torch divides by a Python scalar as a product with its reciprocal)
+    lim = torch.full_like(amax, E4M3_MAX)
+    inv = torch.where(nz, lim / torch.where(nz, amax, torch.ones_like(amax)), torch.zeros_like(amax))
+    q = (w32 * inv[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(E4M3).contiguous()
+    scale = torch.where(nz, amax / lim, torch.ones_like(amax)).contiguous()
+    return q, scale
+
+
+def gemm_e4m3(a_q, a_scale, w_q, w_scale, bias=None, residual=None, geglu=False, out=None, force_bn=0):
+    """out[M,N] = epi((a_q[M,K] @ w_q[N,K]^T) * a_scale[m] * w_scale[n]) with gemm's fp16 epilogue (bias, GEGLU,
+    residual). a_q / w_q: e4m3 (row-strided 2-D views with contiguous last dim); a_scale [M], w_scale [N] fp32."""
+    fn = _optional("b200vton_gemm_e4m3")
+    if a_q.dtype != E4M3 or w_q.dtype != E4M3:
+        raise TypeError(f"gemm_e4m3: operands must be {E4M3}, got {a_q.dtype} and {w_q.dtype}")
+    M, K = a_q.shape
+    N = w_q.shape[0]
+    assert w_q.shape[1] == K and a_q.stride(1) == 1 and w_q.stride(1) == 1
+    assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert a_scale.numel() == M and w_scale.numel() == N
+    n_out = N // 2 if geglu else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=torch.float16, device=a_q.device)
+    assert out.shape == (M, n_out) and out.stride(1) == 1
+    if residual is not None:
+        assert residual.shape == (M, n_out) and residual.stride(1) == 1
+    rc = fn(_p(a_q), a_q.stride(0), _p(a_scale), _p(w_q), w_q.stride(0), _p(w_scale), _p(out), out.stride(0), M, N, K,
+            _p(bias), _p(residual), residual.stride(0) if residual is not None else 0, int(geglu), force_bn, _stream())
+    _check(rc, "b200vton_gemm_e4m3")
     return out
 
 

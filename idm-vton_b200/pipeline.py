@@ -132,6 +132,15 @@ class StableDiffusionXLInpaintPipeline:
             raise ValueError(f"from_pretrained needs explicit components (no hub access): missing {missing}")
         return cls(**components)
 
+    def set_linear_precision(self, precision):
+        """"fp16" (default) or "fp8" for the per-token linears of every transformer block of both UNets (INTEGRATION.md,
+        "FP8 linears"). The UNets re-pack their engines on the next call, which rebuilds the denoiser and its graphs;
+        garment K/V cached under the other precision are dropped."""
+        for m in (self.unet, self.unet_encoder):
+            m.set_linear_precision(precision)
+        if self.garment_cache is not None:
+            self.garment_cache.clear()
+
     def register_to_config(self, **kw):
         for k, v in kw.items():
             setattr(self.config, k, v)

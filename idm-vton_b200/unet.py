@@ -263,6 +263,7 @@ class _UNetBase(nn.Module):
         self._cfg = dict(cfg)
         self._engine = None
         self._lib = None
+        self._linear_precision = "fp16"
         shapes = param_shapes(cfg)
         for k, shp in shapes.items():
             if k.startswith("encoder_hid_proj.") and "encoder_hid_proj" not in self._modules:
@@ -310,8 +311,23 @@ class _UNetBase(nn.Module):
         self._need_lib()
         if self._engine is None:
             self._engine = UNetEngine(self._cfg, self.state_dict(), self.KIND, device=self.device,
-                                      ip_scales=self._ip_scales())
+                                      ip_scales=self._ip_scales(), fp8=self._linear_precision == "fp8")
         return self._engine
+
+    LINEAR_PRECISIONS = ("fp16", "fp8")
+
+    @property
+    def linear_precision(self):
+        return self._linear_precision
+
+    def set_linear_precision(self, precision):
+        """"fp16" (default) or "fp8": the arithmetic of the transformer blocks' per-token linears (attn1 QKV, attn2.to_q,
+        the GEGLU projection), see UNetEngine(fp8=...). A change drops the packed engine; engine() re-packs."""
+        if precision not in self.LINEAR_PRECISIONS:
+            raise ValueError(f"linear precision must be one of {self.LINEAR_PRECISIONS}, got {precision!r}")
+        if precision != self._linear_precision:
+            self._linear_precision = precision
+            self._engine = None
 
     def _apply(self, fn, *a, **k):
         self._engine = None      # weights moved / cast: re-pack lazily

@@ -49,6 +49,16 @@ int b200vton_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, vo
                       int K, const void* bias, const void* residual, int64_t ldr, const void* rowvec,
                       int64_t ld_rowvec, int rows_per_sample, int flags, int force_bn, void* stream);
 
+/* FP8 linear (opt-in, UNetEngine(fp8=True)): out[M,N] = epi((acc * a_scale[m]) * w_scale[n]), acc = A_q[M,K] . W_q[N,K]^T
+ * over e4m3 (float8_e4m3fn) operands with fp32 accumulation; a_scale [M] fp32 per row (token), w_scale [N] fp32 per
+ * output channel (row of W_q). epi is b200vton_gemm_f16's fp16 epilogue on the scaled value: bias, GEGLU (flags & 1, W_q
+ * / w_scale / bias rows tile-interleaved as for b200vton_gemm_f16) and residual, at the same fp16 rounding points; no
+ * other flag. K % 128 == 0; lda / ldw (elements = bytes) multiples of 16; N, ldo, ldr % 8 == 0; A_q, W_q, out, bias,
+ * residual 16-byte aligned, a_scale 4-byte, w_scale 8-byte. force_bn as for b200vton_gemm_f16. */
+int b200vton_gemm_e4m3(const void* A_q, int64_t lda, const void* a_scale, const void* W_q, int64_t ldw,
+                       const void* w_scale, void* out, int64_t ldo, int M, int N, int K, const void* bias,
+                       const void* residual, int64_t ldr, int flags, int force_bn, void* stream);
+
 /* NHWC 3x3 convolution, pad 1, stride 1 or 2, as implicit GEMM: diffusers ResnetBlock2D.conv1/conv2 (+conv_shortcut),
  * conv_in / conv_out (src/unet_hacked_tryon.py:416,755,1245,1386), the conv of Upsample2D, and (stride 2) the conv of
  * Downsample2D (src/unet_block_hacked_tryon.py:1113,1246): the A operand's tensor map then steps two input pixels per
@@ -145,6 +155,13 @@ int b200vton_groupnorm(const void* x0, int C0, const void* x1, int C1, int B, in
  * (src/attentionhacked_garmnet.py:321-322). */
 int b200vton_layernorm(const void* x, int64_t ldx, int rows, int C, const void* gamma, const void* beta, float eps,
                        void* out, int64_t ldo, void* stream);
+
+/* b200vton_layernorm followed by the FP8 linears' row quantization: with y16 the fp16 LayerNorm row (written to out
+ * [rows, ldo] when out is not NULL, bit-identical to b200vton_layernorm), amax = max|y16|, q_scale[r] = amax / 448 and
+ * q[r, :] = e4m3_rn_satfinite(y16 * (448 / amax)) (fp32 IEEE division and product); an all-zero row stores q_scale 1 and
+ * q 0. q: [rows, ldq] e4m3, ldq % 16 == 0; q_scale: [rows] fp32. */
+int b200vton_layernorm_e4m3(const void* x, int64_t ldx, int rows, int C, const void* gamma, const void* beta,
+                            float eps, void* out, int64_t ldo, void* q, int64_t ldq, void* q_scale, void* stream);
 
 /* dst[s,y,x,c_off+c] = src[s % Bs, c, y, x]: NCHW module inputs -> NHWC engine buffer; implements the CFG
  * duplication and the 13-channel concat of src/tryon_pipeline.py:1769,1777 as batch/channel offsets. */
