@@ -2,8 +2,9 @@
 //
 //   * attn1 of src/attentionhacked_tryon.py:334-348 + ip_adapter/attention_processor.py:238-262 — self-attention whose
 //     keys/values are [self tokens ; garment tokens]. Segment 0 = this sample's K/V, segment 1 = the cached garment K/V
-//     of sample (b - kv1_off) % kv1_count; the torch.cat never happens. Query rows are the N self tokens only
-//     (the reference computes and discards the Ng garment query rows).
+//     of sample (b - kv1_off) % kv1_count (+ a device step base), or of the row a device table names per sample (a
+//     pool of hoisted garment K/V shared by slots at different steps); the torch.cat never happens. Query rows are the
+//     N self tokens only (the reference computes and discards the Ng garment query rows).
 //   * CFG-uncond samples (b < kv1_off) see ZERO garment features (src/tryon_pipeline.py:1796): K=V=0, so each of the N1
 //     tokens adds exp(0 - m) to the softmax denominator and nothing to the numerator. Closed form, no KV traffic.
 //   * attn2 (ip_adapter/attention_processor.py:1943-1995, IPAttnProcessor2_0): the text softmax and the IP-token softmax
@@ -43,9 +44,11 @@ struct FlashParams {
   int B, H, Nq, N0, N1;
   int D;          // head dimension: head h occupies columns [h*D, h*D + D)
   int kv1_off;    // segment-1 sample index = (b - kv1_off) % kv1_count; negative => zero K/V closed form
-  int kv1_count;  // segment-1 sample index is taken modulo this count
+  int kv1_count;  // segment-1 sample index is taken modulo this count (with kv1_rows: B1, the rows that exist)
   const int* kv1_base;  // optional device scalar added to the segment-1 sample index (hoisted per-step K/V)
-  int causal;     // key j visible to query i iff j <= i (segment 0 only)
+  const int* kv1_rows;  // optional device table: segment-1 sample index = kv1_rows[b - kv1_off] (negative => zero K/V);
+                        // replaces the modulo and kv1_base (per-slot rows of a pool of hoisted K/V)
+  int causal;    // key j visible to query i iff j <= i (segment 0 only)
   float scale_log2;
   int accumulate;   // out = old + fp16(out_scale * fp16(o)) instead of out = fp16(o)
   float out_scale;
@@ -121,7 +124,7 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       tma_prefetch_desc(&tmV1);
     }
   }
-  // Programmatic dependent launch: Q/K/V (and kv1_base) are written by the previous kernels of the stream
+  // Programmatic dependent launch: Q/K/V (and kv1_base / kv1_rows) are written by the previous kernels of the stream
   pdl_wait();
   __syncthreads();
   pdl_launch_dependents();
@@ -130,7 +133,12 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   int idx1 = -1;
   if (p.N1 > 0) {
     idx1 = b - p.kv1_off;
-    if (idx1 >= 0) idx1 = idx1 % p.kv1_count + (p.kv1_base ? *p.kv1_base : 0);
+    if (idx1 >= 0 && p.kv1_rows) {
+      idx1 = p.kv1_rows[idx1];
+      if (idx1 >= p.kv1_count) idx1 = -1;   // rows outside [0, B1) read nothing: the zero-K/V closed form
+    } else if (idx1 >= 0) {
+      idx1 = idx1 % p.kv1_count + (p.kv1_base ? *p.kv1_base : 0);
+    }
   }
   const bool zero_kv = (p.N1 > 0) && (idx1 < 0);
   const int tiles1 = (p.N1 > 0 && idx1 >= 0) ? ((p.N1 + 127) >> 7) : 0;
@@ -505,10 +513,13 @@ static int flash(const void* q, long long ldq, const void* k0, const void* v0, l
   return kErrUnsupported;
 }
 
-// q: [B, Nq, >=H*64] (row stride ldq); k0/v0: [B, N0, .] (ldkv0); k1/v1: [B1, N1, .] (ldkv1); out: [B, Nq, .] (ldo)
-int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
-              const void* v1, long long ldkv1, void* out, long long ldo, int B, int H, int Nq, int N0, int N1, int B1,
-              int kv1_off, int kv1_mod, const void* kv1_base, float scale, int accumulate, cudaStream_t stream) {
+// q: [B, Nq, >=H*64] (row stride ldq); k0/v0: [B, N0, .] (ldkv0); k1/v1: [B1, N1, .] (ldkv1); out: [B, Nq, .] (ldo).
+// kv1_rows (device int32 [B - kv1_off], or null): sample b >= kv1_off reads segment-1 row kv1_rows[b - kv1_off], in
+// place of kv1_mod / kv1_base.
+static int attn_common(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+                       const void* v1, long long ldkv1, void* out, long long ldo, int B, int H, int Nq, int N0, int N1,
+                       int B1, int kv1_off, int kv1_mod, const void* kv1_base, const void* kv1_rows, float scale,
+                       int accumulate, cudaStream_t stream) {
   VTON_CHECK_ARG(B > 0 && H > 0 && Nq > 0 && N0 > 0 && N1 >= 0, "attn: bad sizes B=%d H=%d Nq=%d N0=%d N1=%d", B, H, Nq, N0, N1);
   VTON_CHECK_ARG(ldq % 8 == 0 && ldkv0 % 8 == 0 && ldo % 8 == 0, "attn: row strides must be multiples of 8");
   VTON_CHECK_ARG(aligned_to(out, 4), "attn: out must be 4-byte aligned (stored two halves at a time)");
@@ -524,12 +535,31 @@ int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long
   p.N1 = N1;
   p.D = 64;
   p.kv1_off = has1 ? kv1_off : (N1 > 0 ? B : 0);
-  p.kv1_count = has1 ? (kv1_mod > 0 ? kv1_mod : B1) : 1;
-  p.kv1_base = has1 ? static_cast<const int*>(kv1_base) : nullptr;
+  p.kv1_count = has1 ? (kv1_rows || kv1_mod <= 0 ? B1 : kv1_mod) : 1;
+  p.kv1_base = has1 && !kv1_rows ? static_cast<const int*>(kv1_base) : nullptr;
+  p.kv1_rows = has1 ? static_cast<const int*>(kv1_rows) : nullptr;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.accumulate = accumulate;
   p.out_scale = 1.f;
   return flash(q, ldq, k0, v0, ldkv0, has1 ? k1 : nullptr, has1 ? v1 : nullptr, ldkv1, B1, out, ldo, p, stream);
+}
+
+int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+              const void* v1, long long ldkv1, void* out, long long ldo, int B, int H, int Nq, int N0, int N1, int B1,
+              int kv1_off, int kv1_mod, const void* kv1_base, float scale, int accumulate, cudaStream_t stream) {
+  return attn_common(q, ldq, k0, v0, ldkv0, k1, v1, ldkv1, out, ldo, B, H, Nq, N0, N1, B1, kv1_off, kv1_mod, kv1_base,
+                     nullptr, scale, accumulate, stream);
+}
+
+int attn_rows_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+                   const void* v1, long long ldkv1, void* out, long long ldo, int B, int H, int Nq, int N0, int N1,
+                   int B1, int kv1_off, const void* kv1_rows, float scale, int accumulate, cudaStream_t stream) {
+  VTON_CHECK_ARG(kv1_rows, "attention_rows: kv1_rows is null");
+  VTON_CHECK_ARG(aligned_to(kv1_rows, 4), "attention_rows: kv1_rows must be 4-byte aligned (int32)");
+  VTON_CHECK_ARG(N1 > 0 && B1 > 0 && k1 && v1, "attention_rows: needs segment-1 K/V (N1=%d, B1=%d)", N1, B1);
+  VTON_CHECK_ARG(kv1_off >= 0 && kv1_off < B, "attention_rows: kv1_off %d outside [0, B=%d)", kv1_off, B);
+  return attn_common(q, ldq, k0, v0, ldkv0, k1, v1, ldkv1, out, ldo, B, H, Nq, N0, N1, B1, kv1_off, 0, nullptr,
+                     kv1_rows, scale, accumulate, stream);
 }
 
 // Decoupled cross-attention of the try-on / garment transformer blocks:

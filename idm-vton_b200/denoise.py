@@ -201,10 +201,52 @@ def ddpm_step_coefficients(scheduler, t):
     return float(b_t ** 0.5), float(inv_sa), float(c0), float(c1), float(sigma)
 
 
+def garment_tokens(tryon, hg, wg):
+    """Ng of every try-on block, in tryon.blocks() order: the garment's tokens at the block's level for a garment latent
+    of hg x wg (the stride-2 convolutions round up)."""
+    n, lvl_tokens = (hg, wg), {}
+    for c in tryon.ch:
+        lvl_tokens[c] = n[0] * n[1]
+        n = ((n[0] - 1) // 2 + 1, (n[1] - 1) // 2 + 1)
+    return [lvl_tokens[b.c] for b in tryon.blocks()]
+
+
+def garment_kv_bytes_per_step(tryon, hg, wg):
+    """Bytes of the hoisted K/V of ONE garment for one denoise step: sum over the try-on blocks of Ng * 2C fp16."""
+    return sum(ng * 2 * b.c * 2 for b, ng in zip(tryon.blocks(), garment_tokens(tryon, hg, wg)))
+
+
+def hoisted_garment_kv(tryon, garment, x_g, ctx_g, t_table, t0, t1, chunk, out):
+    """The hoisted garment passes of the timesteps t_table[t0:t1] for the Bg garments of x_g [Bg,hg,wg,64] / ctx_g
+    (garment.encode_context of their text embeddings): the garment UNet batched over `chunk` timesteps per pass (large-M
+    GEMMs, weights read once per chunk), then the garment K/V projection of every try-on block. out[i]: a contiguous
+    [(t1 - t0) * Bg, Ng, 2C] view that receives block i's K/V in timestep-major order (row (t - t0) * Bg + g). The
+    bits depend only on the garments, the timesteps and the chunking."""
+    Bg = x_g.shape[0]
+    blocks = tryon.blocks()
+    T = t1 - t0
+    for c0 in range(0, T, chunk):
+        n = min(chunk, T - c0)
+        t_rows = t_table[t0 + c0:t0 + c0 + n].repeat_interleave(Bg).contiguous()   # timestep-major rows
+        x_big = x_g.repeat(n, 1, 1, 1)
+        ctx_big = [(kv_t.repeat(n, 1, 1), None) for kv_t, _ in ctx_g]
+        feats = []
+        garment.forward(x_big, garment.time_embedding(t_rows, n * Bg), ctx_big, collect=feats)
+        for i, (blk, f) in enumerate(zip(blocks, feats)):
+            tryon.garment_kv(blk, f, out=out[i][c0 * Bg:(c0 + n) * Bg])
+        del feats, x_big, ctx_big
+
+
+def default_garment_chunk(Bg):
+    """Timesteps per hoisted garment pass: B200VTON_GARMENT_CHUNK when set, else as many as keep a pass at <= 64
+    samples."""
+    return int(__import__("os").environ.get("B200VTON_GARMENT_CHUNK", "0")) or max(1, 64 // max(1, Bg))
+
+
 class GarmentKVCache:
     """LRU cache of hoisted garment K/V across requests (SURVEY.md 8f item 4). One entry = the K/V of ONE garment for every
-    denoise step and every try-on block ([T, Ng, 2C] fp16 per block: 4.7 GB at 768x1024 / 30 steps), keyed by the caller's
-    garment id plus everything the values depend on (timestep list, the garment's latent size). A hit replaces the
+    denoise step and every try-on block ([T, Ng, 2C] fp16 per block: 9.44 GB of K and V at 768x1024 / 30 steps, computed
+    from the shapes), keyed by the caller's garment id plus everything the values depend on (timestep list, the garment's latent size). A hit replaces the
     garment's T garment-UNet passes by device-to-device copies (~2 ms)."""
 
     def __init__(self, max_bytes=16 << 30):   # beside 11 GB of weights and the step's K/V on an 80 GB H100
@@ -405,17 +447,12 @@ class TryOnDenoiser:
         per pass."""
         if self._garment_chunk:
             return self._garment_chunk
-        return max(1, 64 // max(1, getattr(self, "Bg", 1)))
+        return default_garment_chunk(getattr(self, "Bg", 1))
 
     def kv_bytes_per_step(self):
         """Bytes of garment K/V one denoise step keeps resident: sum over the try-on blocks of Bg * Ng * 2C fp16, Ng = the
         garment's tokens at the block's level (from the cloth latents' size)."""
-        ch = self.tryon.ch
-        n, lvl_tokens = (self.hg, self.wg), {}
-        for lvl, c in enumerate(ch):
-            lvl_tokens[c] = n[0] * n[1]
-            n = ((n[0] - 1) // 2 + 1, (n[1] - 1) // 2 + 1)
-        return sum(self.Bg * lvl_tokens[b.c] * 2 * b.c * 2 for b in self.tryon.blocks())
+        return self.Bg * garment_kv_bytes_per_step(self.tryon, self.hg, self.wg)
 
     def precompute_garment(self, win_start=0):
         """The garment-UNet passes of the steps [win_start, win_start + window) of the request (one per timestep), batched,
@@ -425,28 +462,19 @@ class TryOnDenoiser:
             self._precompute_garment(win_start)
 
     def _precompute_garment(self, win_start):
-        L = self.L
         T_all, Bg = self.t_table.numel(), self.Bg
         T = min(self.window, T_all - win_start)
-        blocks = self.tryon.blocks()
+        rows = min(self.window, T_all) * Bg
         gkv = self.gkv_all            # buffers of an earlier same-shaped request are overwritten in place
-        if gkv is not None and gkv[0].shape[0] != min(self.window, T_all) * Bg:
+        if gkv is not None and gkv[0].shape[0] != rows:
             gkv = None
             self._graph = None
         self.gkv_all = None
-        for c0 in range(0, T, self.garment_chunk):
-            n = min(self.garment_chunk, T - c0)
-            t_rows = self.t_table[win_start + c0:win_start + c0 + n].repeat_interleave(Bg).contiguous()   # timestep-major rows
-            x_big = self.x_g.repeat(n, 1, 1, 1)
-            ctx_big = [(kv_t.repeat(n, 1, 1), None) for kv_t, _ in self.ctx_g]
-            feats = []
-            self.garment.forward(x_big, self.garment.time_embedding(t_rows, n * Bg), ctx_big, collect=feats)
-            if gkv is None:
-                gkv = [torch.empty((min(self.window, T_all) * Bg, f.shape[1], 2 * f.shape[2]), dtype=torch.float16,
-                                   device=self.device) for f in feats]
-            for i, (blk, f) in enumerate(zip(blocks, feats)):
-                self.tryon.garment_kv(blk, f, out=gkv[i][c0 * Bg:(c0 + n) * Bg])
-            del feats, x_big, ctx_big
+        if gkv is None:
+            gkv = [torch.empty((rows, ng, 2 * b.c), dtype=torch.float16, device=self.device)
+                   for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, self.hg, self.wg))]
+        hoisted_garment_kv(self.tryon, self.garment, self.x_g, self.ctx_g, self.t_table, win_start, win_start + T,
+                           self.garment_chunk, [g[:T * Bg] for g in gkv])
         self.gkv_all = gkv
         self.win_start = win_start
 
@@ -557,19 +585,35 @@ class SlotDenoiser:
     gathers each slot's timestep / coefficient / input-scale row from the per-step tables into the static buffers, with
     copies issued outside the graph (with B200VTON_PDL_GRAPH every kernel node of the graph is a library kernel).
 
-    The garment passes stay in the step: slots at different phases cannot share K/V hoisted over all steps of one request
-    (kv_bytes_per_step x T per garment), so GarmentKVCache does not apply here. Idle slots hold zeros and the identity
-    coefficient row (identity_step_row); their outputs are ignored. No row of one slot enters another slot's result, so at
-    a fixed S a request's result does not depend on which slot it runs in or on what the other slots hold."""
+    Two modes:
+      * pages=None (default): the garment UNet runs inside the step at batch S with per-slot timesteps, and the garment
+        features of slot s are streamed into try-on rows s / S + s. Nothing is hoisted.
+      * pages=P (pool mode, P >= S): the hoisted garment K/V of whole garments live in a pool of P pages, one tensor
+        [P*T, Ng, 2C] per try-on block (page p = rows p*T .. p*T + T - 1, so one TMA map per block covers every page and
+        the captured graph stays valid while pages are refilled). fill_page runs the T garment passes of one garment
+        alone (Bg = 1, TryOnDenoiser's default chunking, hoisted_garment_kv), so a page's bits depend only on the garment
+        and the timesteps. The step is the try-on UNet only: slot s reads row page(s)*T + step(s) of the pool through
+        b200vton_attention_rows, and an idle slot reads row -1, the zero-K/V closed form (no K/V traffic, and no
+        unwritten memory is ever read). The caller (ContinuousTryOnServer) decides which garment is in which page.
+
+    Idle slots hold zeros and the identity coefficient row (identity_step_row); their outputs are ignored. No row of one
+    slot enters another slot's result, so at a fixed S a request's result does not depend on which slot it runs in or on
+    what the other slots hold."""
 
     PDL_IN_GRAPH = TryOnDenoiser.PDL_IN_GRAPH
     capture = TryOnDenoiser.capture
 
-    def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots):
+    def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots, pages=None):
         self.tryon, self.garment = tryon, garment
         self.L = tryon.L
         self.device = tryon.device
         self.S = int(slots)
+        self.P = None if pages is None else int(pages)
+        if self.P is not None and self.P < self.S:
+            raise ValueError(f"pool mode needs at least one garment K/V page per slot: {self.P} pages for {self.S} slots")
+        self.garment_chunk = default_garment_chunk(1)
+        self.page = [None] * self.S                 # pool mode: the page each slot's request reads
+        self.pool = None
         self._graph = None
         self._key = None
         self.ctx_t = None
@@ -578,6 +622,8 @@ class SlotDenoiser:
         names = ["b200vton_cfg_ddpm_step_rows" if kind == "ddpm" else "b200vton_cfg_solver_step_rows"]
         if kind == "euler":
             names.append("b200vton_nchw_to_nhwc_scaled_rows")
+        if self.P is not None:
+            names.append("b200vton_attention_rows")
         return names
 
     def configure(self, scheduler, timesteps, h, w, guidance_scale=2.0, do_cfg=True, eta=0.0, guidance_rescale=0.0):
@@ -603,7 +649,7 @@ class SlotDenoiser:
         self.kind, self.do_cfg, self.h, self.w = kind, bool(do_cfg), h, w
         S = self.S
         self.Bt = 2 * S if do_cfg else S
-        key = (S, h, w, self.do_cfg, kind)
+        key = (S, h, w, self.do_cfg, kind) + (() if self.P is None else (self.P, self.T))
         if key != self._key:
             self._key = key
             self._graph = None
@@ -613,8 +659,17 @@ class SlotDenoiser:
             self.noise = torch.zeros_like(self.latents)
             self.x0_prev = torch.zeros_like(self.latents) if kind == "dpmpp" else None
             self.x_t = torch.zeros((self.Bt, h, w, CIN_PAD), dtype=f16, device=dev)
-            self.x_g = torch.zeros((S, h, w, CIN_PAD), dtype=f16, device=dev)
-            self.t_g = torch.zeros(S, dtype=f32, device=dev)
+            if self.P is None:
+                self.x_g = torch.zeros((S, h, w, CIN_PAD), dtype=f16, device=dev)
+                self.t_g = torch.zeros(S, dtype=f32, device=dev)
+            else:
+                # allocated once (the old pool is released first); every page is written by fill_page before a slot's
+                # row names it
+                self.x_g = self.t_g = self.pool = None
+                self.pool = [torch.empty((self.P * self.T, ng, 2 * b.c), dtype=f16, device=dev)
+                             for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, h, w))]
+                self.rows = torch.full((S,), -1, dtype=torch.int32, device=dev)
+                self.page = [None] * S
             self.t_t = torch.zeros(self.Bt, dtype=f32, device=dev)
             self.coef = torch.zeros((S, 8), dtype=f32, device=dev)
             self.scale = torch.ones(S, dtype=f32, device=dev)
@@ -626,21 +681,54 @@ class SlotDenoiser:
         idx = torch.tensor([self.T if i is None else int(i) for i in steps], dtype=torch.long).to(self.device)
         torch.index_select(self.coef_table, 0, idx, out=self.coef)
         t = self.t_table.index_select(0, idx)
-        self.t_g.copy_(t)
+        if self.t_g is not None:
+            self.t_g.copy_(t)
         self.t_t.copy_(t.repeat(self.Bt // self.S))
         if self.scale_table is not None:
             torch.index_select(self.scale_table, 0, idx, out=self.scale)
+        if self.P is not None:
+            # pool mode: slot s reads row page(s) * T + step(s) of the pool, an idle slot row -1 (zero K/V)
+            rows = []
+            for s, i in enumerate(steps):
+                if i is not None and self.page[s] is None:
+                    raise ValueError(f"slot {s} is at step {i} but holds no garment K/V page")
+                rows.append(-1 if i is None else self.page[s] * self.T + int(i))
+            if any(not -1 <= r < self.P * self.T for r in rows):
+                raise ValueError(f"garment K/V rows {rows} outside [-1, {self.P * self.T})")
+            self.rows.copy_(torch.tensor(rows, dtype=torch.int32))
+
+    def fill_page(self, p, cloth_latents, text_embeds_cloth):
+        """Pool mode: writes the garment K/V of all T steps of one garment (cloth_latents [1,4,h,w], text_embeds_cloth
+        [1,77,X]) into page p: its T garment-UNet passes at Bg = 1, chunked as TryOnDenoiser chunks them, so the page
+        holds the bits TryOnDenoiser's gkv_all holds for that garment alone. Runs eagerly (not in the step graph)."""
+        if self.P is None or self.pool is None:
+            raise RuntimeError("SlotDenoiser.fill_page needs pool mode (pages=P) and configure() first")
+        if not 0 <= p < self.P:
+            raise ValueError(f"page {p} outside [0, {self.P})")
+        if tuple(cloth_latents.shape[-2:]) != (self.h, self.w):
+            raise ValueError(f"cloth_latents has spatial size {tuple(cloth_latents.shape[-2:])}, the server's latents "
+                             f"{(self.h, self.w)}")
+        dev, f16, T = self.device, torch.float16, self.T
+        with nvtx_range(f"b200vton.garment_page_fill[{p}]"):
+            x_g = torch.zeros((1, self.h, self.w, CIN_PAD), dtype=f16, device=dev)
+            self.L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), x_g, c_off=0)
+            ctx_g = self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16))
+            hoisted_garment_kv(self.tryon, self.garment, x_g, ctx_g, self.t_table, 0, T, self.garment_chunk,
+                               [g[p * T:(p + 1) * T] for g in self.pool])
 
     def _rows(self, s):
         return (s, self.S + s) if self.do_cfg else (s,)
 
     def admit(self, s, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
-              add_time_ids, image_embeds, text_embeds_cloth):
+              add_time_ids, image_embeds, text_embeds_cloth, page=None):
         """Writes one request into slot s, and only its rows. latents [1,4,h,w]; mask [1,1,h,w]; masked_image_latents,
         pose_latents, cloth_latents [1,4,h,w]; prompt_embeds [n,77,X], add_text_embeds [n,P], add_time_ids [n,6],
         image_embeds [n,16,X] with n = 2 ([uncond ; cond]) under CFG, else 1 (mask, masked_image_latents and
-        pose_latents may have n rows too); text_embeds_cloth [1,77,X]."""
+        pose_latents may have n rows too); text_embeds_cloth [1,77,X]. Pool mode: `page` is the filled page of the
+        request's garment (cloth_latents and text_embeds_cloth are then not read)."""
         L, dev, f16 = self.L, self.device, torch.float16
+        if self.P is not None and (page is None or not 0 <= page < self.P):
+            raise ValueError(f"pool mode: admit needs the page of the request's garment in [0, {self.P}), got {page}")
         for name, t in (("latents", latents), ("mask", mask), ("masked_image_latents", masked_image_latents),
                         ("pose_latents", pose_latents), ("cloth_latents", cloth_latents)):
             if tuple(t.shape[-2:]) != (self.h, self.w):
@@ -651,9 +739,10 @@ class SlotDenoiser:
             self.ctx_t = [(torch.zeros((self.Bt, prompt_embeds.shape[1], 2 * b.c), dtype=f16, device=dev),
                            torch.zeros((self.Bt, ni, 2 * b.c), dtype=f16, device=dev) if ni else None)
                           for b in self.tryon.blocks()]
-            self.ctx_g = [(torch.zeros((self.S, text_embeds_cloth.shape[1], 2 * b.c), dtype=f16, device=dev), None)
-                          for b in self.garment.blocks()]
-            self.aug = torch.zeros((self.Bt, self.tryon.ae[2].shape[0]), dtype=f16, device=dev)
+            if self.P is None:
+                self.ctx_g = [(torch.zeros((self.S, text_embeds_cloth.shape[1], 2 * b.c), dtype=f16, device=dev), None)
+                              for b in self.garment.blocks()]
+            self.aug =torch.zeros((self.Bt, self.tryon.ae[2].shape[0]), dtype=f16, device=dev)
             self._graph = None
         self.latents[s].copy_(latents[0].to(dev, f16))
         for j, r in enumerate(rows):
@@ -665,19 +754,24 @@ class SlotDenoiser:
                                       out=[(kt[r:r + 1], None if ki is None else ki[r:r + 1]) for kt, ki in self.ctx_t])
             self.tryon.aug_embedding(add_text_embeds[j:j + 1].to(dev, f16), add_time_ids[j:j + 1].to(dev),
                                      out=self.aug[r:r + 1])
-        L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), self.x_g[s:s + 1], c_off=0)
-        self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16), out=[(kv[s:s + 1], None) for kv, _ in self.ctx_g])
+        if self.P is None:
+            L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), self.x_g[s:s + 1], c_off=0)
+            self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16),
+                                        out=[(kv[s:s + 1], None) for kv, _ in self.ctx_g])
+        else:
+            self.page[s] = int(page)
         if self.x0_prev is not None:
             self.x0_prev[s].zero_()
 
     def release(self, s):
         """Frees slot s: its latents, state and input channels go back to zeros (the context rows keep finite values
-        that no other slot reads)."""
+        that no other slot reads); in pool mode it no longer names a page."""
         for buf in (self.latents, self.latents_next, self.noise, self.x0_prev, self.x_g):
             if buf is not None:
                 buf[s].zero_()
         for r in self._rows(s):
             self.x_t[r].zero_()
+        self.page[s] = None
 
     def _launch_step(self):
         """The launch sequence of one step over the slot buffers (graph-capturable)."""
@@ -686,10 +780,15 @@ class SlotDenoiser:
             L.nchw_to_nhwc_scaled_rows(self.latents, self.x_t, self.scale, c_off=0)
         else:
             L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)
-        feats = []
-        self.garment.forward(self.x_g, self.garment.time_embedding(self.t_g, S), self.ctx_g, collect=feats)
-        temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
-        self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=S if self.do_cfg else 0)
+        if self.P is None:
+            feats = []
+            self.garment.forward(self.x_g, self.garment.time_embedding(self.t_g, S), self.ctx_g, collect=feats)
+            temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
+            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=S if self.do_cfg else 0)
+        else:                                           # the try-on UNet only: each slot reads its page's row
+            temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
+            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, n_persons=S if self.do_cfg else 0,
+                                          gkv_pre=(self.pool, self.rows))
         if self.kind == "ddpm":
             L.cfg_ddpm_step_rows(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
         else:

@@ -321,7 +321,9 @@ class UNetEngine:
     def _block(self, blk, h, B, N, ctx, gfeat, n_persons, collect, gkv_pre=None):
         """h: [B*N, C]. gfeat: garment feature for this block ([Bg,Ng,C], try-on fast path), a full [B,Ng,C] tensor
         (reference-format features through the module seam) or None (garment UNet). gkv_pre = (kv [T*Bg,Ng,2C],
-        n_garments, step_base int32 device scalar): garment K/V precomputed for all denoise steps."""
+        n_garments, step_base int32 device scalar): garment K/V precomputed for all denoise steps; or (pool [P*T,Ng,2C],
+        rows int32 device [B - n_persons]): a pool of hoisted K/V pages, person sample j reading row rows[j] (negative:
+        zero K/V, an idle slot)."""
         L = self.L
         C, H = blk.c, blk.heads
         f8 = blk.fp8
@@ -341,7 +343,10 @@ class UNetEngine:
         else:
             qkv = L.gemm(n1, blk.wqkv).view(B, N, 3 * C)
         q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
-        if gkv_pre is not None:
+        if gkv_pre is not None and len(gkv_pre) == 2:
+            pool, rows = gkv_pre
+            a = L.attention_rows(q, k, v, pool[..., :C], pool[..., C:], rows, kv1_off=n_persons, heads=H)
+        elif gkv_pre is not None:
             kv_all, n_g, base = gkv_pre
             a = L.attention(q, k, v, kv_all[..., :C], kv_all[..., C:], kv1_off=n_persons, heads=H, kv1_mod=n_g,
                             kv1_base=base)
@@ -388,7 +393,7 @@ class UNetEngine:
             gf = state["gfeats"][i] if state["gfeats"] is not None else None
             gp = None
             if state["gkv_pre"] is not None:
-                gp = (state["gkv_pre"][0][i], state["gkv_pre"][1], state["gkv_pre"][2])
+                gp = (state["gkv_pre"][0][i], *state["gkv_pre"][1:])
             h = self._block(blk, h, B, N, state["ctx"][i], gf, state["n_persons"], state["collect"], gp)
             state["idx"] = i + 1
         out = L.gemm(h, t.wout, bias=t.bout, residual=x.view(B * N, C))

@@ -48,13 +48,16 @@ SIGNATURES = {
 }
 
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
-# step kernels of the continuous-batching denoiser and the FP8 linears. `has_symbol` tells whether a binding can use them.
+# step kernels of the continuous-batching denoiser, the FP8 linears and the per-sample-row attention of its pool mode.
+# `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
     "b200vton_cfg_solver_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "b200vton_nchw_to_nhwc_scaled_rows": [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp],
     "b200vton_gemm_e4m3": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _i64, _i, _i, _vp],
     "b200vton_layernorm_e4m3": [_vp, _i64, _i, _i, _vp, _vp, _f, _vp, _i64, _vp, _i64, _vp, _vp],
+    "b200vton_attention_rows": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp,
+                                _f, _i, _vp],
 }
 _present = set()
 
@@ -237,6 +240,30 @@ def attention(q, k0, v0, k1=None, v1=None, n1=0, kv1_off=0, heads=None, scale=No
                                 out.stride(1), B, H, Nq, N0, n1, B1, kv1_off, kv1_mod, _p(kv1_base), float(scale),
                                 int(accumulate), _stream())
     _check(rc, "b200vton_attention")
+    return out
+
+
+def attention_rows(q, k0, v0, k1, v1, kv1_rows, kv1_off=0, heads=None, scale=None, accumulate=False, out=None):
+    """attention with one segment-1 row per sample: sample b >= kv1_off reads row kv1_rows[b - kv1_off] of k1/v1
+    [B1,N1,*]; a negative row takes the zero-K/V closed form. kv1_rows: int32 CUDA tensor of B - kv1_off entries."""
+    fn = _optional("b200vton_attention_rows")
+    B, Nq = q.shape[0], q.shape[1]
+    N0 = k0.shape[1]
+    assert q.stride(2) == 1 and k0.stride(2) == 1 and v0.stride(2) == 1
+    assert q.stride(0) == Nq * q.stride(1) and k0.stride(0) == N0 * k0.stride(1) and v0.stride() == k0.stride()
+    B1, n1, ld1 = k1.shape[0], k1.shape[1], k1.stride(1)
+    assert k1.stride(2) == 1 and k1.stride(0) == n1 * ld1 and v1.stride() == k1.stride()
+    if kv1_rows.dtype != torch.int32 or not kv1_rows.is_cuda or not kv1_rows.is_contiguous() or \
+            kv1_rows.numel() != B - kv1_off:
+        raise ValueError(f"attention_rows: kv1_rows must be a contiguous CUDA int32 tensor of B - kv1_off = "
+                         f"{B - kv1_off} entries, got {kv1_rows.dtype} {tuple(kv1_rows.shape)} on {kv1_rows.device}")
+    if scale is None:
+        scale = 64 ** -0.5
+    if out is None:
+        out = torch.empty((B, Nq, heads * 64), dtype=torch.float16, device=q.device)
+    rc = fn(_p(q), q.stride(1), _p(k0), _p(v0), k0.stride(1), _p(k1), _p(v1), ld1, _p(out), out.stride(1), B, heads, Nq,
+            N0, n1, B1, kv1_off, _p(kv1_rows), float(scale), int(accumulate), _stream())
+    _check(rc, "b200vton_attention_rows")
     return out
 
 

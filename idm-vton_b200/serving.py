@@ -158,8 +158,18 @@ class ContinuousTryOnServer:
 
     One scheduler (the pipeline's), one `num_inference_steps` and one guidance scale for every request, and one person
     size (height x width); the garment must have the same latent size. Garments are VAE-encoded once per garment_id
-    exactly as TryOnServer does. The garment UNet runs inside every step at batch `slots` (no hoisting and no
-    GarmentKVCache: requests at different phases need the garment K/V of different timesteps).
+    exactly as TryOnServer does.
+
+    Garment work, two modes:
+      * garment_kv_bytes=None (default): the garment UNet runs inside every step at batch `slots` (no hoisting and no
+        GarmentKVCache: requests at different phases need the garment K/V of different timesteps).
+      * garment_kv_bytes=N (pool mode): a pool of P = N // page_bytes pages of hoisted garment K/V (SlotDenoiser with
+        pages=P), page_bytes = T * kv_bytes_per_step of one garment (9.44 GB at 768x1024 with 30 steps, computed from the
+        shapes). Admitting a request pins its garment's page; on a miss the garment's T passes fill a free page, or the
+        least recently used unpinned one, eagerly at admission before that step's replay. Slots with the same garment
+        share its page; a retired request unpins it and the page stays resident, so a later request for that garment
+        runs no garment pass at all. The step is then the try-on UNet only. P < slots is refused (ValueError naming the
+        page size) before any launch. `stats` counts garment_page_fills and garment_page_hits.
 
     RNG: each request owns a generator seeded with `req.seed` (the server's seed when None; unseeded when both are None)
     and draws in the order the pipeline draws for a batch of one: the initial noise, the masked image's VAE sample, the
@@ -169,10 +179,11 @@ class ContinuousTryOnServer:
     own (requests finishing at the same step share one VAE decode).
     `eta`: DDIM's eta, as the pipeline's `__call__` takes it (0 = deterministic DDIM, 1 = DDPM-like variance).
     Refused: guidance_rescale (not a parameter here), schedulers other than DDPM / DDIM / Euler / DPM-Solver++, and a
-    library without the per-slot step kernels (NotImplementedError naming the symbol, before any launch)."""
+    library without the per-slot step kernels or, in pool mode, without b200vton_attention_rows (NotImplementedError
+    naming the symbol, before any launch)."""
 
     def __init__(self, pipe, height=1024, width=768, slots=4, num_inference_steps=30, guidance_scale=2.0, seed=None,
-                 output_type="pt", eta=0.0):
+                 output_type="pt", eta=0.0, garment_kv_bytes=None):
         self.pipe = pipe
         self.height, self.width = height, width
         self.S = int(slots)
@@ -187,6 +198,10 @@ class ContinuousTryOnServer:
         self.slots = [None] * self.S                 # per slot: dict(req, gen, step) or None
         self.garments = {}
         self.den = None
+        self.garment_kv_bytes = None if garment_kv_bytes is None else int(garment_kv_bytes)
+        self.page_of = collections.OrderedDict()     # pool mode: garment_id -> page, least recently admitted first
+        self.pins = collections.Counter()            # pool mode: page -> slots whose request reads it
+        self.free_pages = []
         self.last_latents = {}                       # ticket -> final latents of the requests the last step() finished
         self._next_ticket = 0
         self.stats = collections.Counter()
@@ -213,9 +228,30 @@ class ContinuousTryOnServer:
         return len(self.waiting) + sum(e is not None for e in self.slots)
 
     # ---------------------------------------------------------------------------------------------
-    def _make_denoiser(self):
+    def _make_denoiser(self, pages=None):
         from .denoise import SlotDenoiser
-        return SlotDenoiser(self.pipe.unet.engine(), self.pipe.unet_encoder.engine(), self.S)
+        return SlotDenoiser(self.pipe.unet.engine(), self.pipe.unet_encoder.engine(), self.S, pages=pages)
+
+    def page_bytes(self, T=None):
+        """Pool mode: bytes of one garment's page, the hoisted K/V of all T steps at Bg = 1 (from the shapes)."""
+        from .denoise import garment_kv_bytes_per_step
+        T = self.num_inference_steps if T is None else T
+        return T * garment_kv_bytes_per_step(self.pipe.unet.engine(), *self.latent_size)
+
+    def _pages(self, T):
+        """Pool mode: the number of pages the budget holds; refuses fewer than one per slot."""
+        page = self.page_bytes(T)
+        P = self.garment_kv_bytes // page
+        if P < self.S:
+            raise ValueError(f"garment_kv_bytes={self.garment_kv_bytes} holds {P} garment K/V pages of {page} bytes "
+                             f"({page / 1e9:.2f} GB: {T} steps at latent size {self.latent_size}); pool mode needs at "
+                             f"least one page per slot ({self.S}, i.e. {self.S * page} bytes)")
+        return P
+
+    def _reset_pages(self, P):
+        self.page_of.clear()
+        self.pins.clear()
+        self.free_pages = list(range(P))
 
     def _configure(self):
         """Timesteps and per-step tables of the run (the pipeline's own timestep selection at strength 1); checks every
@@ -227,7 +263,12 @@ class ContinuousTryOnServer:
         timesteps, n = pipe.get_timesteps(n, 1.0, pipe._execution_device)
         self.timesteps = timesteps
         if self.den is None:
-            self.den = self._make_denoiser()
+            if self.garment_kv_bytes is None:
+                self.den = self._make_denoiser()
+            else:
+                P = self._pages(len(timesteps))
+                self.den = self._make_denoiser(pages=P)
+                self._reset_pages(P)
         self.den.configure(pipe.scheduler, timesteps, *self.latent_size, guidance_scale=self.guidance_scale,
                            do_cfg=pipe.do_classifier_free_guidance, eta=self.eta, guidance_rescale=self.guidance_rescale)
         self.T = self.den.T
@@ -297,10 +338,31 @@ class ContinuousTryOnServer:
             seed = self._seed(req)
             gen = torch.Generator(device).manual_seed(seed) if seed is not None else None
             prep = self._prepare_request(req, gen)
+            page = None if self.garment_kv_bytes is None else self._pin_page(req.garment_id, g)
             self.den.admit(s, cloth_latents=g["latents"], image_embeds=g["image_embeds"],
-                           text_embeds_cloth=g["text_embeds_cloth"], **prep)
-            self.slots[s] = dict(req=req, gen=gen, step=0)
+                           text_embeds_cloth=g["text_embeds_cloth"], page=page, **prep)
+            self.slots[s] = dict(req=req, gen=gen, step=0, page=page)
             self.stats["admitted"] += 1
+
+    def _pin_page(self, gid, g):
+        """Pool mode: the page holding garment `gid`, pinned for one more slot. A miss fills a free page, else the least
+        recently admitted unpinned one (one exists: a free slot means at most slots - 1 pinned pages, and P >= slots)."""
+        p = self.page_of.get(gid)
+        if p is not None:
+            self.page_of.move_to_end(gid)
+            self.stats["garment_page_hits"] += 1
+        else:
+            if self.free_pages:
+                p = self.free_pages.pop(0)
+            else:
+                victim = next(k for k, q in self.page_of.items() if self.pins[q] == 0)
+                p = self.page_of.pop(victim)
+                self.stats["garment_page_evictions"] += 1
+            self.den.fill_page(p, g["latents"], g["text_embeds_cloth"])
+            self.page_of[gid] = p
+            self.stats["garment_page_fills"] += 1
+        self.pins[p] += 1
+        return p
 
     def _decode(self, latents):
         if self.output_type == "latent":
@@ -342,6 +404,8 @@ class ContinuousTryOnServer:
         images = self._decode(final)
         for s in done:
             den.release(s)
+            if self.slots[s]["page"] is not None:      # the page stays resident as a cache entry
+                self.pins[self.slots[s]["page"]] -= 1
             self.slots[s] = None
         self.stats["images"] += len(done)
         return {t: images[i] for i, t in enumerate(tickets)}

@@ -87,6 +87,16 @@ int b200vton_attention(const void* q, int64_t ldq, const void* k0, const void* v
                        int B1, int kv1_off, int kv1_mod, const void* kv1_base, float scale, int accumulate,
                        void* stream);
 
+/* b200vton_attention with one segment-1 row per sample: sample b >= kv1_off reads row kv1_rows[b - kv1_off] of the
+ * [B1, N1, *] K/V (kv1_rows: device int32 [B - kv1_off], read after the previous kernel of the stream completes, so a
+ * captured graph can be replayed with a table rewritten before each replay). A negative entry, or one >= B1, selects
+ * the all-zero K/V closed form of the samples b < kv1_off: no K/V is read for it. Lets slots at different denoise steps
+ * share one pool of hoisted garment K/V (one page of T rows per garment). Needs segment-1 K/V (N1 > 0, B1 > 0, k1, v1)
+ * and 0 <= kv1_off < B; otherwise the arguments and results of b200vton_attention. */
+int b200vton_attention_rows(const void* q, int64_t ldq, const void* k0, const void* v0, int64_t ldkv0, const void* k1,
+                            const void* v1, int64_t ldkv1, void* out, int64_t ldo, int B, int H, int Nq, int N0, int N1,
+                            int B1, int kv1_off, const void* kv1_rows, float scale, int accumulate, void* stream);
+
 /* Decoupled cross-attention (attn2 of every transformer block) in one launch:
  *   out = fp16( fp16(softmax(Q Kt^T * scale) Vt) + fp16(ip_scale * fp16(softmax(Q Ki^T * scale) Vi)) ),  head_dim 64,
  * Kt/Vt = [B, Nt <= 80, *] the text tokens (attn2.to_k / to_v), Ki/Vi = [B, Ni <= 16, *] the IP-Adapter image tokens

@@ -1,18 +1,24 @@
 """Continuous batching against batch mode on one GPU, at config-2 geometry (768x1024, DDPM 30 steps, guidance 2.0) with
 random SDXL-shaped weights as bench.py builds them.
 
-A seeded Poisson arrival trace of `--requests` requests over `--garments` garments goes through
-serving.TryOnServer(max_batch=S) and through serving.ContinuousTryOnServer(slots=S), alternated in one process
-(`--rounds` rounds after a warm-up of each). Every round starts each mode afresh: a new server, a new denoiser, an
-empty garment K/V cache of `--cache-gb` for batch mode. So each round's numbers include the capture of its CUDA graphs
-(the continuous denoiser captures one graph, at its first step; batch mode's denoiser captures one per batch shape and
-again whenever a batch of another size follows, as it does in service). The rate is `--load` times the capacity of a
-continuous server at full occupancy, measured first. Prints one JSON line with, per mode:
+A seeded Poisson arrival trace of `--requests` requests over `--garments` garments goes through three modes, alternated
+in one process (`--rounds` rounds after a warm-up of each):
+  batch:            serving.TryOnServer(max_batch=S) with a garment K/V cache of `--kv-gb`;
+  continuous:       serving.ContinuousTryOnServer(slots=S), the garment UNet inside every step;
+  continuous_pool:  serving.ContinuousTryOnServer(slots=S, garment_kv_bytes=--kv-gb), hoisted garment K/V pages.
+Batch mode's cache and the pool get the same budget (one garment's K/V of all 30 steps is 9.44 GB, so the default 40 GB
+holds 4 garments). Every round starts each mode afresh: a new server, a new denoiser, an empty cache or pool. So each
+round's numbers include the capture of its CUDA graphs (a continuous denoiser captures one graph, at its first step;
+batch mode's denoiser captures one per batch shape and again whenever a batch of another size follows, as it does in
+service) and, in pool mode, every page fill. The rate is `--load` times the capacity of a default continuous server at
+full occupancy, measured first. Prints one JSON line with, per mode:
   images_per_s:   requests / (last image - first arrival);
   latency_s:      p50 / p95 from arrival to image;
-and the step time at full occupancy (the continuous step graph at S slots) against the batch-mode step at batch S with
-one garment plus its hoisted garment passes per step; the card's name and power limit, read in the same run.
-Usage: python scripts/continuous_timing.py [--slots 4] [--requests 32] [--garments 8] [--rounds 2]"""
+  (pool mode) garment_page_fills / garment_page_hits and the hit rate;
+and the step time at full occupancy (the default continuous step graph and the pool step graph at S slots) against the
+batch-mode step at batch S with one garment plus its hoisted garment passes per step; the time of one page fill (a
+miss); the card's name and power limit, read in the same run.
+Usage: python scripts/continuous_timing.py [--slots 4] [--requests 32] [--garments 8] [--rounds 2] [--kv-gb 40]"""
 import argparse
 import json
 import os
@@ -85,8 +91,10 @@ def main():
     ap.add_argument("--garments", type=int, default=8)
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--load", type=float, default=0.9)
-    ap.add_argument("--cache-gb", type=int, default=16, help="batch mode's garment K/V cache")
+    ap.add_argument("--kv-gb", type=float, default=40,
+                    help="garment K/V budget of batch mode's cache and of the pool (GB, 1e9 bytes)")
     args = ap.parse_args()
+    kv_bytes = int(args.kv_gb * 1e9)
     from idm_vton_b200 import lib as L
     from idm_vton_b200.denoise import TryOnDenoiser
     from idm_vton_b200.engine import SDXL_GARMENT, SDXL_TRYON
@@ -117,6 +125,32 @@ def main():
     cont_step = e0.elapsed_time(e1) / 10
     del cont
     torch.cuda.empty_cache()
+    # the same for pool mode (S garments filled at admission), then the time of one page fill
+    pool = ContinuousTryOnServer(pipe, height=H, width=W, slots=S, num_inference_steps=T, guidance_scale=2.0, seed=7,
+                                 garment_kv_bytes=kv_bytes)
+    reqs = make_requests(S, S, dev, seed=1)
+    for r in reqs:
+        pool.submit(r)
+    pool.step()
+    e0, e1 = ev(), ev()
+    e0.record()
+    for _ in range(10):
+        pool.den.step([5] * S)
+    e1.record()
+    torch.cuda.synchronize()
+    pool_step = e0.elapsed_time(e1) / 10
+    g = pool.garments[reqs[0].garment_id]
+    fills = []
+    for _ in range(3):
+        e0, e1 = ev(), ev()
+        e0.record()
+        pool.den.fill_page(pool.den.P - 1, g["latents"], g["text_embeds_cloth"])
+        e1.record()
+        torch.cuda.synchronize()
+        fills.append(e0.elapsed_time(e1))
+    out["pool"] = dict(pages=pool.den.P, page_bytes=pool.page_bytes(), fill_ms=[round(f, 1) for f in fills])
+    del pool, g
+    torch.cuda.empty_cache()
     req = bench.synth_request(SDXL_TRYON, SDXL_GARMENT, S, H // 8, W // 8, seed=42, device=dev, garments=1)
     den = TryOnDenoiser(unet.engine(), unet_enc.engine())
     sch = DDPMScheduler()
@@ -134,7 +168,8 @@ def main():
     torch.cuda.synchronize()
     batch_garment, batch_step = e0.elapsed_time(e1), e1.elapsed_time(e2) / 10
     del den
-    out["step_ms"] = dict(continuous_full=round(cont_step, 2), batch=round(batch_step, 2),
+    out["step_ms"] = dict(continuous_full=round(cont_step, 2), continuous_pool_full=round(pool_step, 2),
+                          batch=round(batch_step, 2),
                           batch_garment_passes_per_step=round(batch_garment / T, 2),
                           batch_total=round(batch_step + batch_garment / T, 2))
 
@@ -148,9 +183,11 @@ def main():
     out["arrival_rate_per_s"] = round(rate, 3)
     modes = {
         "batch": lambda: TryOnServer(pipe, height=H, width=W, num_inference_steps=T, guidance_scale=2.0, max_batch=S,
-                                     seed=7, garment_cache_bytes=args.cache_gb << 30),
+                                     seed=7, garment_cache_bytes=kv_bytes),
         "continuous": lambda: ContinuousTryOnServer(pipe, height=H, width=W, slots=S, num_inference_steps=T,
                                                     guidance_scale=2.0, seed=7),
+        "continuous_pool": lambda: ContinuousTryOnServer(pipe, height=H, width=W, slots=S, num_inference_steps=T,
+                                                         guidance_scale=2.0, seed=7, garment_kv_bytes=kv_bytes),
     }
     import gc
 
@@ -170,13 +207,20 @@ def main():
         srv.run()
         del srv
     res = {n: [] for n in modes}
+    pages = []
     for _ in range(args.rounds):
         for name in modes:
-            res[name].append(serve(fresh(name), make_requests(args.requests, args.garments, dev, seed=5), arrivals))
+            srv = fresh(name)
+            res[name].append(serve(srv, make_requests(args.requests, args.garments, dev, seed=5), arrivals))
+            if name == "continuous_pool":
+                pages.append((srv.stats["garment_page_fills"], srv.stats["garment_page_hits"]))
+            del srv
     for name, runs in res.items():
         out[name] = dict(images_per_s=[round(r[0], 3) for r in runs],
                          latency_p50_s=[round(pct(r[1], 50), 2) for r in runs],
                          latency_p95_s=[round(pct(r[1], 95), 2) for r in runs])
+    out["continuous_pool"].update(garment_page_fills=[f for f, _ in pages], garment_page_hits=[h for _, h in pages],
+                                  hit_rate=[round(h / max(1, f + h), 3) for f, h in pages])
     out["card_after"] = card()
     print(json.dumps(out))
 
