@@ -8,9 +8,12 @@ try-on UNet (batch 2B), applies CFG and the DDPM update. Here one step is a fixe
 captured once in a CUDA graph and replayed per step; step-invariant work (cross-attention K/V of text / IP tokens,
 aug_emb, the static input channels) is hoisted to prepare().
 """
+import collections
+
 import torch
 
 from .engine import CIN_PAD, UNetEngine
+from .scheduler import DPMSolverMultistepScheduler, _init_step_index, config_getter, solver_order_at
 
 
 class nvtx_range:
@@ -46,9 +49,11 @@ def scheduler_kind(scheduler):
     return "ddpm"
 
 
-def _config_getter(scheduler):
-    cfg = getattr(scheduler, "config", None)
-    return (lambda k, d=None: cfg.get(k, d)) if isinstance(cfg, dict) else (lambda k, d=None: getattr(cfg, k, d))
+def check_guidance_rescale(scheduler, guidance_rescale):
+    """Refuses guidance_rescale > 0 with any step but DDPM's: the guidance rescale is fused with the DDPM step only."""
+    if guidance_rescale > 0 and scheduler_kind(scheduler) != "ddpm":
+        raise NotImplementedError(f"guidance_rescale with {type(scheduler).__name__}: the engine's guidance rescale is "
+                                  "fused with the DDPM step only")
 
 
 def ddim_step_coefficients(scheduler, t, eta=0.0):
@@ -56,7 +61,7 @@ def ddim_step_coefficients(scheduler, t, eta=0.0):
     b200vton_cfg_solver_step), computed in fp32 torch like diffusers 0.25 from the generic attributes:
     `alphas_cumprod`, `final_alpha_cumprod` (or `config.set_alpha_to_one`), `config.num_train_timesteps` and
     `num_inference_steps`. The step goes to t - T_train // num_inference_steps."""
-    get = _config_getter(scheduler)
+    get = config_getter(getattr(scheduler, "config", None))
     if get("prediction_type", "epsilon") != "epsilon" or get("clip_sample", False) or get("thresholding", False):
         raise NotImplementedError("the fused DDIM step covers epsilon prediction without clip_sample / thresholding")
     ac = scheduler.alphas_cumprod.to(device="cpu", dtype=torch.float32)
@@ -79,10 +84,7 @@ def _run_indices(scheduler, timesteps):
     `_init_step_index` (the second match when it occurs twice), then one further per step."""
     sched = scheduler.timesteps.detach().cpu().to(torch.float64)
     run = [float(t) for t in timesteps]
-    idx = (sched == run[0]).nonzero().flatten().tolist()
-    if not idx:
-        raise ValueError(f"timestep {run[0]} is not in {type(scheduler).__name__}.timesteps")
-    start = idx[1] if len(idx) > 1 else idx[0]
+    start = _init_step_index(sched, run[0])
     if sched[start:start + len(run)].tolist() != run:
         raise ValueError("the run's timesteps must be consecutive entries of the scheduler's timesteps")
     return list(range(start, start + len(run)))
@@ -91,7 +93,7 @@ def _run_indices(scheduler, timesteps):
 def euler_step_tables(scheduler, timesteps):
     """([(s, inv_a, p, q, r, sigma_n, k)], [input scale]) per step of EulerDiscreteScheduler at s_churn = 0 (the
     pipeline passes no s_churn), in fp32 torch like diffusers 0.25, from `sigmas` (N + 1 values) and `timesteps`."""
-    get = _config_getter(scheduler)
+    get = config_getter(getattr(scheduler, "config", None))
     if get("prediction_type", "epsilon") != "epsilon" or get("interpolation_type", "linear") != "linear":
         raise NotImplementedError("the fused Euler step covers epsilon prediction with linear sigma interpolation")
     sig = scheduler.sigmas.detach().to(device="cpu", dtype=torch.float32)
@@ -107,8 +109,7 @@ def dpmpp_step_coefficients_table(scheduler, timesteps):
     """[(s, inv_a, p, q, r, sigma_n, k)] per step of DPMSolverMultistepScheduler (dpmsolver++, midpoint, order 1 / 2),
     in fp32 torch like diffusers 0.25, from `sigmas`, `timesteps` and the config's solver_order, lower_order_final and
     euler_at_final; k = 1 / r0 at second-order steps and 0 at first-order ones."""
-    from .scheduler import solver_order_at
-    get = _config_getter(scheduler)
+    get = config_getter(getattr(scheduler, "config", None))
     if get("solver_order", 2) not in (1, 2):
         raise NotImplementedError(f"solver_order {get('solver_order')}: the fused DPM-Solver++ step covers orders 1 and 2")
     if get("algorithm_type", "dpmsolver++") != "dpmsolver++":
@@ -120,21 +121,17 @@ def dpmpp_step_coefficients_table(scheduler, timesteps):
                                   "use_lu_lambdas")
     sig = scheduler.sigmas.detach().to(device="cpu", dtype=torch.float32)
     n = len(scheduler.timesteps)
-
-    def alpha_sigma(i):
-        alpha = 1 / ((sig[i] ** 2 + 1) ** 0.5)
-        return alpha, sig[i] * alpha
-
+    alpha_sigma = DPMSolverMultistepScheduler._sigma_to_alpha_sigma_t
     rows = []
     for j, i in enumerate(_run_indices(scheduler, timesteps)):
-        alpha_t, sigma_t = alpha_sigma(i)
-        alpha_n, sigma_n = alpha_sigma(i + 1)
+        alpha_t, sigma_t = alpha_sigma(sig[i])
+        alpha_n, sigma_n = alpha_sigma(sig[i + 1])
         lam = torch.log(alpha_t) - torch.log(sigma_t)
         h = torch.log(alpha_n) - torch.log(sigma_n) - lam
         c = alpha_n * (torch.exp(-h) - 1.0)
         k = 0.0
         if solver_order_at(j, i, n, scheduler.config) == 2:
-            alpha_p, sigma_p = alpha_sigma(i - 1)
+            alpha_p, sigma_p = alpha_sigma(sig[i - 1])
             r0 = (lam - (torch.log(alpha_p) - torch.log(sigma_p))) / h
             k = float(1.0 / r0)
         rows.append((float(sigma_t), float(torch.tensor(1.0) / alpha_t), float(sigma_n / sigma_t), float(-c), 0.0, 0.0, k))
@@ -169,8 +166,7 @@ def ddpm_step_coefficients(scheduler, t):
     kernel implements epsilon prediction with fixed_small variance and no clipping / thresholding: anything else raises.
     A custom timestep list (`custom_timesteps`) needs `previous_timestep`: the even spacing t - T_train // steps would
     be wrong for it."""
-    cfg = getattr(scheduler, "config", None)
-    get = (lambda k, d=None: cfg.get(k, d)) if isinstance(cfg, dict) else (lambda k, d=None: getattr(cfg, k, d))
+    get = config_getter(getattr(scheduler, "config", None))
     if get("prediction_type", "epsilon") != "epsilon" or get("variance_type", "fixed_small") != "fixed_small" \
             or get("clip_sample", False) or get("thresholding", False):
         raise NotImplementedError("the fused CFG+DDPM step covers epsilon prediction, fixed_small variance, no "
@@ -199,6 +195,51 @@ def ddpm_step_coefficients(scheduler, t):
     sigma = var ** 0.5 if t > 0 else torch.tensor(0.0)
     inv_sa = torch.tensor(1.0, dtype=torch.float32) / (a_t ** 0.5)
     return float(b_t ** 0.5), float(inv_sa), float(c0), float(c1), float(sigma)
+
+
+def identity_step_row(kind):
+    """The coefficient row of an idle slot of SlotDenoiser: the step returns its latents unchanged (zeros stay zeros),
+    whatever the finite eps. DDPM {gs, sb, inv_sa, c0, c1, sigma, phi, 0}: x0 = 0, prev = 1 * x; DDIM and DPM-Solver++
+    {gs, s, inv_a, p, q, r, sigma_n, k}: x0 = x, out = fp16(1 * x0) (DDIM) or 1 * x + fp16(0 * x0) (DPM++); Euler:
+    x0 = x - 0, d = 0, out = x + 0."""
+    return {"ddpm": [0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0],
+            "ddim": [0.0, 0.0, 1.0, 0.0, 1.0, 0.0, 0.0, 0.0],
+            "euler": [0.0] * 8,
+            "dpmpp": [0.0, 0.0, 1.0, 1.0, 0.0, 0.0, 0.0, 0.0]}[kind]
+
+
+class StepPlan(collections.namedtuple("StepPlan", "kind coef_table t_table scale_table step_draws noise_applied T")):
+    """The per-step tables of one run (step_plan), in the layout the step kernels read. coef_table [T + 1, 8] fp32: row
+    i = the coefficients of step i, {gs, sb, inv_sa, c0, c1, sigma, phi, 0} for DDPM and {gs, s, inv_a, p, q, r,
+    sigma_n, k} of b200vton_cfg_solver_step otherwise; row T = the idle row (identity_step_row). t_table [T + 1] fp32:
+    the timesteps (fractional for Euler's linspace spacing), 0 at row T. scale_table [T + 1] fp32: Euler's input
+    scales, 1 at row T; None for the other kinds. step_draws, noise_applied: as solver_step_tables. T: steps in the run."""
+
+    def to(self, device):
+        return self._replace(coef_table=self.coef_table.to(device), t_table=self.t_table.to(device),
+                             scale_table=None if self.scale_table is None else self.scale_table.to(device))
+
+
+def step_plan(scheduler, timesteps, guidance_scale, guidance_rescale=0.0, eta=0.0):
+    """The StepPlan of a run of `scheduler` over `timesteps` (solver_step_tables, with DDIM's `eta`) at guidance scale gs
+    and guidance rescale phi (DDPM only: check_guidance_rescale)."""
+    check_guidance_rescale(scheduler, guidance_rescale)
+    kind, coefs, scales, draws, applied = solver_step_tables(scheduler, timesteps, eta)
+    gs = float(guidance_scale)
+    rows = [[gs, *c, float(guidance_rescale), 0.0] if kind == "ddpm" else [gs, *c] for c in coefs]
+    f32 = torch.float32
+    return StepPlan(kind, torch.tensor(rows + [identity_step_row(kind)], dtype=f32),
+                    torch.tensor([float(t) for t in timesteps] + [0.0], dtype=f32),
+                    None if scales is None else torch.tensor(list(scales) + [1.0], dtype=f32), draws, applied, len(coefs))
+
+
+def variance_noise(den, i, shape, generator, device, dtype):
+    """The variance noise of step i for a denoiser's `step`, or None. It is drawn from `generator` when the scheduler's own
+    `step` would draw it (DDPM at t > 0, DDIM at eta > 0, Euler at every step: den.step_draws), so the generator ends
+    in the reference's state, and dropped when the update does not apply it (Euler's: den.noise_applied)."""
+    from .pipeline import randn_tensor
+    noise = randn_tensor(shape, generator=generator, device=device, dtype=dtype) if den.step_draws[i] else None
+    return noise if den.noise_applied else None
 
 
 def garment_tokens(tryon, hg, wg):
@@ -250,7 +291,6 @@ class GarmentKVCache:
     garment's T garment-UNet passes by device-to-device copies (~2 ms)."""
 
     def __init__(self, max_bytes=16 << 30):   # beside 11 GB of weights and the step's K/V on an 80 GB H100
-        import collections
         self.max_bytes = int(max_bytes)
         self.entries = collections.OrderedDict()
         self.bytes = 0
@@ -282,7 +322,105 @@ class GarmentKVCache:
         self.bytes = 0
 
 
-class TryOnDenoiser:
+def _describe(x):
+    """(address, shape, dtype) of a tensor, element-wise through the lists and tuples that hold per-block buffers."""
+    if isinstance(x, torch.Tensor):
+        return x.data_ptr(), x.shape, x.dtype
+    if isinstance(x, (list, tuple)):
+        return tuple(_describe(v) for v in x)
+    return x
+
+
+class _CapturedStep:
+    """The step of the module docstring over static buffers, launched eagerly or replayed from a CUDA graph, as
+    TryOnDenoiser and SlotDenoiser share it. Subclasses supply the garment K/V the try-on UNet reads (_gkv_pre; None:
+    the garment UNet runs in the step) and the per-step uploads (_upload). ROWS: one coefficient row per sample."""
+
+    ROWS = False
+    # Programmatic dependent launch INSIDE the captured step only (B200VTON_PDL_GRAPH, default below): every kernel node
+    # of the graph is one of this library's kernels, which call griddepcontrol.wait before they touch global
+    # memory, so the set-up of kernel n+1 overlaps the tail of kernel n. Eager launches, which interleave with cuBLAS /
+    # cuDNN / ATen kernels in the pipeline call, keep plain stream order unless B200VTON_PDL=1 asks otherwise.
+    # Default: ON inside the graph, OFF for eager launches.
+    PDL_IN_GRAPH = __import__("os").environ.get("B200VTON_PDL_GRAPH", "1") == "1"
+    _graph = _graph_sig = None   # the captured step and the _signature it was captured at
+
+    def _signature(self):
+        """What a captured step bakes in: the kernel selection and the address, shape and dtype of every buffer the
+        graph reads or writes (not of those it allocates while capturing, such as eps)."""
+        gkv_pre = self._gkv_pre()
+        garment = (self.x_g, self.t_g, self.ctx_g) if gkv_pre is None else gkv_pre
+        return (self.kind, self.rescale, self.do_cfg, gkv_pre is not None) + _describe(
+            [self.latents, self.latents_next, self.noise, self.x0_prev, self.x_t, self.t_t, self.coef, self.scale,
+             self.aug, self.ctx_t, garment])
+
+    def _launch_step(self):
+        """The launch sequence of one denoise step over the static buffers (graph-capturable)."""
+        L = self.L
+        if self.kind == "euler":                                  # scale_model_input on the latent channels only
+            scatter = L.nchw_to_nhwc_scaled_rows if self.ROWS else L.nchw_to_nhwc_scaled
+            scatter(self.latents, self.x_t, self.scale, c_off=0)
+        else:
+            L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)      # CFG duplication + channel concat as offsets
+        gkv_pre, feats = self._gkv_pre(), None
+        if gkv_pre is None:
+            feats = []
+            self.garment.forward(self.x_g, self.garment.time_embedding(self.t_g, self.x_g.shape[0]), self.ctx_g,
+                                 collect=feats)
+        temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
+        self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, gkv_pre=gkv_pre,
+                                      n_persons=self.latents.shape[0] if self.do_cfg else 0)
+        if self.kind == "ddpm":
+            step = L.cfg_ddpm_step_rows if self.ROWS else L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
+            step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
+        else:
+            step = L.cfg_solver_step_rows if self.ROWS else L.cfg_solver_step
+            step(self.eps, self.latents, self.noise if self.kind == "ddim" else None, self.coef, self.kind,
+                 x0_prev=self.x0_prev, do_cfg=self.do_cfg, out=self.latents_next)
+        self.latents.copy_(self.latents_next)
+
+    def capture(self):
+        """Capture one step into a CUDA graph (one warm-up launch on a side stream, then one recorded pass)."""
+        self._graph = self._graph_sig = None                      # the old graph's memory goes before the new one's
+        s = torch.cuda.Stream(device=self.device)
+        s.wait_stream(torch.cuda.current_stream())
+        keep = self.latents.clone()
+        keep_x0 = self.x0_prev.clone() if self.kind == "dpmpp" else None     # the warm-up step advances the state
+        with torch.cuda.stream(s):
+            self._launch_step()
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        pdl_before = self.L.get_option("programmatic_launch", 0)
+        if self.PDL_IN_GRAPH:
+            self.L.set_option("programmatic_launch", 1)
+        try:
+            with torch.cuda.graph(g):
+                self._launch_step()
+        finally:
+            if self.PDL_IN_GRAPH:
+                self.L.set_option("programmatic_launch", pdl_before)
+        self.latents.copy_(keep)
+        if keep_x0 is not None:
+            self.x0_prev.copy_(keep_x0)
+        self._graph, self._graph_sig = g, self._signature()
+
+    def _run(self, use_graph, name, *rows):
+        """One step: _upload(*rows), then a replay of the graph (re-captured if its _signature changed) or the eager
+        launches. The signature is read first: an upload may wait for the device, and this overlaps the running step."""
+        stale = use_graph and self._graph_sig != self._signature()
+        self._upload(*rows)
+        with nvtx_range(name):
+            if stale:
+                self.capture()
+            if use_graph:
+                self._graph.replay()
+            else:
+                self._launch_step()
+        return self.latents
+
+
+class TryOnDenoiser(_CapturedStep):
     def __init__(self, tryon: UNetEngine, garment: UNetEngine, hoist_garment=True, garment_chunk=None, max_kv_bytes=None):
         """max_kv_bytes: budget for the resident garment K/V of the hoisted passes (default: 60% of the free device memory
         when the step tables are set). When all denoise steps do not fit (e.g. 1024x1024, 50 steps, batch 4 = 84 GB),
@@ -297,7 +435,6 @@ class TryOnDenoiser:
         self.garment = garment
         self.L = tryon.L
         self.device = tryon.device
-        self._graph = None
         self.hoist_garment = hoist_garment
         if garment_chunk is None:
             garment_chunk = int(__import__("os").environ.get("B200VTON_GARMENT_CHUNK", "0")) or None
@@ -317,12 +454,9 @@ class TryOnDenoiser:
         with Bt = 2B under CFG ([uncond ; cond] order, src/tryon_pipeline.py:1711-1714); cloth_latents [Bg,4,hg,wg],
         text_embeds_cloth [Bg,77,X]. The garment may have a latent size of its own: the garment UNet runs at the cloth's
         size (src/tryon_pipeline.py:1654,1787) and its Ng tokens per level join the try-on attention as they are."""
-        torch.cuda.nvtx.range_push("b200vton.prepare(context K/V, aug_emb, static input channels)")
-        try:
+        with nvtx_range("b200vton.prepare(context K/V, aug_emb, static input channels)"):
             self._prepare(latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
                           add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg, guidance_rescale)
-        finally:
-            torch.cuda.nvtx.range_pop()
 
     def _prepare(self, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
                  add_time_ids, image_embeds, text_embeds_cloth, guidance_scale, do_cfg, guidance_rescale):
@@ -338,7 +472,6 @@ class TryOnDenoiser:
             if tuple(t.shape[-2:]) != (h, w):
                 raise ValueError(f"{name} has spatial size {tuple(t.shape[-2:])}, the latents {(h, w)}: the try-on UNet "
                                  "input concatenates them along channels")
-        # the rescale flag selects the step's last kernel: a graph captured with the other one must not be replayed
         rescale = bool(do_cfg) and guidance_rescale > 0
         key = (B, Bt, Bg, h, w, hg, wg, bool(do_cfg), rescale, tuple(prompt_embeds.shape), tuple(image_embeds.shape),
                tuple(text_embeds_cloth.shape))
@@ -349,24 +482,23 @@ class TryOnDenoiser:
         self.do_cfg = do_cfg
         self.guidance_scale = float(guidance_scale)
         self.rescale = rescale
-        self.guidance_rescale = float(guidance_rescale)
+        self.guidance_rescale = float(guidance_rescale) if rescale else 0.0     # phi applies under CFG only
         if fresh:
             # (re)allocate every static buffer the step graph points at; same-shaped requests reuse them (and the
             # captured graph) and only overwrite their contents
-            self._graph = None
             self.gkv_all = None
             self.latents = torch.empty((B, 4, h, w), dtype=f16, device=dev)
             self.latents_next = torch.empty_like(self.latents)
             self.noise = torch.zeros_like(self.latents)
             self.x_t = torch.zeros((Bt, h, w, CIN_PAD), dtype=f16, device=dev)
             self.x_g = torch.zeros((Bg, hg, wg, CIN_PAD), dtype=f16, device=dev)   # the garment at its own size
-            self.t_dev = torch.zeros(1, dtype=torch.float32, device=dev)
+            self.t_t = self.t_g = torch.zeros(1, dtype=torch.float32, device=dev)  # one timestep for both UNets
             self.coef = torch.zeros(8, dtype=torch.float32, device=dev)
-            self.in_scale = torch.ones(1, dtype=torch.float32, device=dev)     # Euler's scale_model_input
+            self.scale = torch.ones(1, dtype=torch.float32, device=dev)        # Euler's scale_model_input
             self.x0_prev = None                                                # DPM-Solver++ state
             self.step_base = torch.zeros(1, dtype=torch.int32, device=dev)   # step index * Bg (hoisted garment K/V)
             self.ctx_t = self.ctx_g = self.aug = None
-            self.eps = None
+            self._graph = self._graph_sig = self.eps = None    # the old graph's memory goes before the K/V budget is read
         self.latents.copy_(latents.to(dev, f16))
         L.nchw_to_nhwc(mask.to(dev, f16).contiguous(), self.x_t, c_off=4)
         L.nchw_to_nhwc(masked_image_latents.to(dev, f16).contiguous(), self.x_t, c_off=5)
@@ -377,31 +509,18 @@ class TryOnDenoiser:
         self.aug = self.tryon.aug_embedding(add_text_embeds.to(dev, f16), add_time_ids.to(dev), out=self.aug)
 
     def set_step_tables(self, scheduler, timesteps, garment_keys=None, cache=None, eta=0.0):
-        """Uploads the per-step scalars: t (fp32, fractional for Euler's linspace spacing) and the step kernel's
-        coefficients — {gs, sqrt(1-abar), 1/sqrt(abar), c0, c1, sigma, phi} for DDPM, {gs, s, inv_a, p, q, r, sigma_n, k}
-        of b200vton_cfg_solver_step for DDIM (with `eta`), Euler and DPM-Solver++ (solver_step_tables) — then runs the
-        hoisted garment passes. The scheduler kind selects the step's last kernel: switching kinds drops the captured
-        graph. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments whose
-        K/V of all steps are cached are copied in instead of recomputed — valid only when the caller guarantees that a
+        """Uploads the run's step_plan (timesteps and the step kernel's coefficients, DDIM with `eta`), then runs the
+        hoisted garment passes. garment_keys (one hashable per garment of this batch) + cache (GarmentKVCache): garments
+        whose K/V of all steps are cached are copied in instead of recomputed — valid only when the caller guarantees that a
         key identifies (cloth latents, text_embeds_cloth); the timestep list and the garment's latent size are added to
         the key here (the person's size does not enter the garment K/V)."""
-        kind, coefs, scales, self.step_draws, self.noise_applied = solver_step_tables(scheduler, timesteps, eta)
-        if kind != "ddpm" and self.rescale:
-            raise NotImplementedError("guidance_rescale is implemented for DDPMScheduler only")
-        if kind != getattr(self, "kind", None):
-            self.kind = kind
-            self._graph = None
-        if kind == "dpmpp":
+        plan = step_plan(scheduler, timesteps, self.guidance_scale, self.guidance_rescale, eta)
+        vars(self).update(plan.to(self.device)._asdict())                  # kind, coef_table, ..., T
+        if self.kind == "dpmpp":
             if self.x0_prev is None:
                 self.x0_prev = torch.zeros_like(self.latents)
-                self._graph = None
             self.x0_prev.zero_()
-        rows = [[self.guidance_scale, *c, self.guidance_rescale, 0.0] if kind == "ddpm" else [self.guidance_scale, *c]
-                for c in coefs]
-        self.coef_table = torch.tensor(rows, dtype=torch.float32, device=self.device)
-        self.scale_table = None if scales is None else torch.tensor(scales, dtype=torch.float32, device=self.device)
-        self.t_table = torch.tensor([float(t) for t in timesteps], dtype=torch.float32, device=self.device)
-        T = len(rows)
+        T = self.T
         self.window = T
         if self.hoist_garment:
             budget = self.max_kv_bytes
@@ -429,7 +548,6 @@ class TryOnDenoiser:
                         # entries' geometry instead of re-running the garment passes; the step graph is captured afterwards
                         self.gkv_all = [torch.empty((T * self.Bg, *src.shape[1:]), dtype=src.dtype, device=self.device)
                                         for src in hit[0]]
-                        self._graph = None
                     for g, e in enumerate(hit):                         # timestep-major rows: row = t * Bg + g
                         for dst, src in zip(self.gkv_all, e):
                             dst.view(T, self.Bg, *dst.shape[1:])[:, g].copy_(src)
@@ -462,13 +580,12 @@ class TryOnDenoiser:
             self._precompute_garment(win_start)
 
     def _precompute_garment(self, win_start):
-        T_all, Bg = self.t_table.numel(), self.Bg
+        T_all, Bg = self.T, self.Bg
         T = min(self.window, T_all - win_start)
         rows = min(self.window, T_all) * Bg
         gkv = self.gkv_all            # buffers of an earlier same-shaped request are overwritten in place
         if gkv is not None and gkv[0].shape[0] != rows:
             gkv = None
-            self._graph = None
         self.gkv_all = None
         if gkv is None:
             gkv = [torch.empty((rows, ng, 2 * b.c), dtype=torch.float16, device=self.device)
@@ -478,104 +595,29 @@ class TryOnDenoiser:
         self.gkv_all = gkv
         self.win_start = win_start
 
-    # -------------------------------------------------------------------------------------------
-    def _launch_step(self):
-        """The launch sequence of one denoise step over the static buffers (graph-capturable)."""
-        L = self.L
-        if self.kind == "euler":                                  # scale_model_input on the latent channels only
-            L.nchw_to_nhwc_scaled(self.latents, self.x_t, self.in_scale, c_off=0)
-        else:
-            L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)      # CFG duplication + channel concat as offsets
-        temb_t = self.tryon.time_embedding(self.t_dev, self.Bt, self.aug)
-        n_persons = self.B if self.do_cfg else 0
-        if self.gkv_all is not None:
-            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, n_persons=n_persons,
-                                          gkv_pre=(self.gkv_all, self.Bg, self.step_base))
-        else:
-            feats = []
-            temb_g = self.garment.time_embedding(self.t_dev, self.Bg)
-            self.garment.forward(self.x_g, temb_g, self.ctx_g, collect=feats)
-            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=n_persons)
-        if self.kind == "ddpm":
-            step = L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
-            step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
-        else:
-            L.cfg_solver_step(self.eps, self.latents, self.noise if self.kind == "ddim" else None, self.coef, self.kind,
-                              x0_prev=self.x0_prev, do_cfg=self.do_cfg, out=self.latents_next)
-        self.latents.copy_(self.latents_next)
-
-    # Programmatic dependent launch INSIDE the captured step only (B200VTON_PDL_GRAPH, default below): every kernel node
-    # of the graph is one of this library's kernels, which call griddepcontrol.wait before they touch global
-    # memory, so the set-up of kernel n+1 overlaps the tail of kernel n. Eager launches, which interleave with cuBLAS /
-    # cuDNN / ATen kernels in the pipeline call, keep plain stream order unless B200VTON_PDL=1 asks otherwise.
-    # Default: ON inside the graph, OFF for eager launches.
-    PDL_IN_GRAPH = __import__("os").environ.get("B200VTON_PDL_GRAPH", "1") == "1"
-
-    def capture(self):
-        """Capture one step into a CUDA graph (after a warm-up launch on a side stream)."""
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream())
-        keep = self.latents.clone()
-        keep_x0 = self.x0_prev.clone() if self.kind == "dpmpp" else None     # the warm-up step advances the state
-        with torch.cuda.stream(s):
-            self._launch_step()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        pdl_before = self.L.get_option("programmatic_launch", 0)
-        if self.PDL_IN_GRAPH:
-            self.L.set_option("programmatic_launch", 1)
-        try:
-            with torch.cuda.graph(g):
-                self._launch_step()
-        finally:
-            if self.PDL_IN_GRAPH:
-                self.L.set_option("programmatic_launch", pdl_before)
-        self.latents.copy_(keep)
-        if keep_x0 is not None:
-            self.x0_prev.copy_(keep_x0)
-        self._graph = g
+    def _gkv_pre(self):
+        """Hoisted: each try-on block reads the Bg rows from step_base on of its resident garment K/V."""
+        return None if self.gkv_all is None else (self.gkv_all, self.Bg, self.step_base)
 
     def step(self, i, noise=None, use_graph=True):
         """Runs denoise step i (tables from set_step_tables). noise: [B,4,h,w] fp16 variance noise or None."""
         if self.hoist_garment and self.gkv_all is not None and (i // self.window) * self.window != self.win_start:
             self.precompute_garment((i // self.window) * self.window)      # next K/V window (budgeted hoisting)
-        self.t_dev.copy_(self.t_table[i:i + 1])
+        return self._run(use_graph, "b200vton.denoise_step", i, noise)
+
+    def _upload(self, i, noise):
+        self.t_t.copy_(self.t_table[i:i + 1])
         self.coef.copy_(self.coef_table[i])
         self.step_base.copy_(self.base_table[i:i + 1])
         if self.scale_table is not None:
-            self.in_scale.copy_(self.scale_table[i:i + 1])
+            self.scale.copy_(self.scale_table[i:i + 1])
         if noise is not None:
             self.noise.copy_(noise)
         else:
             self.noise.zero_()
-        with nvtx_range("b200vton.denoise_step"):
-            if use_graph:
-                if self._graph is None:
-                    self.capture()
-                    self.t_dev.copy_(self.t_table[i:i + 1])
-                    self.coef.copy_(self.coef_table[i])
-                    self.step_base.copy_(self.base_table[i:i + 1])
-                    if self.scale_table is not None:
-                        self.in_scale.copy_(self.scale_table[i:i + 1])
-                self._graph.replay()
-            else:
-                self._launch_step()
-        return self.latents
 
 
-def identity_step_row(kind):
-    """The coefficient row of an idle slot of SlotDenoiser: the step returns its latents unchanged (zeros stay zeros),
-    whatever the finite eps. DDPM {gs, sb, inv_sa, c0, c1, sigma, phi, 0}: x0 = 0, prev = 1 * x; DDIM and DPM-Solver++
-    {gs, s, inv_a, p, q, r, sigma_n, k}: x0 = x, out = fp16(1 * x0) (DDIM) or 1 * x + fp16(0 * x0) (DPM++); Euler:
-    x0 = x - 0, d = 0, out = x + 0."""
-    return {"ddpm": [0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0],
-            "ddim": [0.0, 0.0, 1.0, 0.0, 1.0, 0.0, 0.0, 0.0],
-            "euler": [0.0] * 8,
-            "dpmpp": [0.0, 0.0, 1.0, 1.0, 0.0, 0.0, 0.0, 0.0]}[kind]
-
-
-class SlotDenoiser:
+class SlotDenoiser(_CapturedStep):
     """The denoise step of continuous batching: S slots, each holding one request at its own step index.
 
     Every buffer is indexed by slot: [S, ...] for persons and garments, [2S, ...] for the try-on batch under CFG (uncond
@@ -600,8 +642,8 @@ class SlotDenoiser:
     slot enters another slot's result, so at a fixed S a request's result does not depend on which slot it runs in or on
     what the other slots hold."""
 
-    PDL_IN_GRAPH = TryOnDenoiser.PDL_IN_GRAPH
-    capture = TryOnDenoiser.capture
+    ROWS = True
+    rescale = False              # refused by configure: the rescale kernel reads one coefficient row for the batch
 
     def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots, pages=None):
         self.tryon, self.garment = tryon, garment
@@ -614,7 +656,6 @@ class SlotDenoiser:
         self.garment_chunk = default_garment_chunk(1)
         self.page = [None] * self.S                 # pool mode: the page each slot's request reads
         self.pool = None
-        self._graph = None
         self._key = None
         self.ctx_t = None
 
@@ -634,30 +675,23 @@ class SlotDenoiser:
         if guidance_rescale and guidance_rescale > 0:
             raise NotImplementedError("guidance_rescale > 0 is not supported by continuous batching: the rescale kernel "
                                       "reads one coefficient row for the whole batch")
-        kind, coefs, scales, self.step_draws, self.noise_applied = solver_step_tables(scheduler, timesteps, eta)
-        for name in self._needs(kind):
+        plan = step_plan(scheduler, timesteps, guidance_scale, eta=eta)    # row T: idle slots
+        for name in self._needs(plan.kind):
             if not self.L.has_symbol(name):
                 raise NotImplementedError(f"continuous batching needs {name}, which this library binding does not export")
-        gs = float(guidance_scale)
-        rows = [[gs, *c, 0.0, 0.0] if kind == "ddpm" else [gs, *c] for c in coefs]
-        rows.append(identity_step_row(kind))                       # row T: idle slots
+        vars(self).update(plan.to(self.device)._asdict())                  # kind, coef_table, ..., T
         dev, f16, f32 = self.device, torch.float16, torch.float32
-        self.T = len(coefs)
-        self.coef_table = torch.tensor(rows, dtype=f32, device=dev)
-        self.t_table = torch.tensor([float(t) for t in timesteps] + [0.0], dtype=f32, device=dev)
-        self.scale_table = None if scales is None else torch.tensor(list(scales) + [1.0], dtype=f32, device=dev)
-        self.kind, self.do_cfg, self.h, self.w = kind, bool(do_cfg), h, w
+        self.do_cfg, self.h, self.w = bool(do_cfg), h, w
         S = self.S
         self.Bt = 2 * S if do_cfg else S
-        key = (S, h, w, self.do_cfg, kind) + (() if self.P is None else (self.P, self.T))
+        key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T))
         if key != self._key:
             self._key = key
-            self._graph = None
             self.ctx_t = self.ctx_g = self.aug = None
             self.latents = torch.zeros((S, 4, h, w), dtype=f16, device=dev)
             self.latents_next = torch.zeros_like(self.latents)
             self.noise = torch.zeros_like(self.latents)
-            self.x0_prev = torch.zeros_like(self.latents) if kind == "dpmpp" else None
+            self.x0_prev = torch.zeros_like(self.latents) if self.kind == "dpmpp" else None
             self.x_t = torch.zeros((self.Bt, h, w, CIN_PAD), dtype=f16, device=dev)
             if self.P is None:
                 self.x_g = torch.zeros((S, h, w, CIN_PAD), dtype=f16, device=dev)
@@ -743,7 +777,6 @@ class SlotDenoiser:
                 self.ctx_g = [(torch.zeros((self.S, text_embeds_cloth.shape[1], 2 * b.c), dtype=f16, device=dev), None)
                               for b in self.garment.blocks()]
             self.aug =torch.zeros((self.Bt, self.tryon.ae[2].shape[0]), dtype=f16, device=dev)
-            self._graph = None
         self.latents[s].copy_(latents[0].to(dev, f16))
         for j, r in enumerate(rows):
             x = self.x_t[r:r + 1]
@@ -773,43 +806,18 @@ class SlotDenoiser:
             self.x_t[r].zero_()
         self.page[s] = None
 
-    def _launch_step(self):
-        """The launch sequence of one step over the slot buffers (graph-capturable)."""
-        L, S = self.L, self.S
-        if self.kind == "euler":                        # scale_model_input with each slot's own sigma
-            L.nchw_to_nhwc_scaled_rows(self.latents, self.x_t, self.scale, c_off=0)
-        else:
-            L.nchw_to_nhwc(self.latents, self.x_t, c_off=0)
-        if self.P is None:
-            feats = []
-            self.garment.forward(self.x_g, self.garment.time_embedding(self.t_g, S), self.ctx_g, collect=feats)
-            temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
-            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, n_persons=S if self.do_cfg else 0)
-        else:                                           # the try-on UNet only: each slot reads its page's row
-            temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
-            self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, n_persons=S if self.do_cfg else 0,
-                                          gkv_pre=(self.pool, self.rows))
-        if self.kind == "ddpm":
-            L.cfg_ddpm_step_rows(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
-        else:
-            L.cfg_solver_step_rows(self.eps, self.latents, self.noise if self.kind == "ddim" else None, self.coef,
-                                   self.kind, x0_prev=self.x0_prev, do_cfg=self.do_cfg, out=self.latents_next)
-        self.latents.copy_(self.latents_next)
+    def _gkv_pre(self):
+        return None if self.P is None else (self.pool, self.rows)
 
     def step(self, steps, noises=None, use_graph=True):
         """One denoise step of every occupied slot. steps: per slot, its request's step index or None (idle); noises:
         {slot: [1,4,h,w] variance noise} for the slots whose scheduler step applies one. Returns the latents [S,4,h,w]."""
         if self.ctx_t is None:
             raise RuntimeError("SlotDenoiser.step before any admission")
+        return self._run(use_graph, "b200vton.slot_denoise_step", steps, noises)
+
+    def _upload(self, steps, noises):
         self.gather(steps)
         self.noise.zero_()
         for s, n in (noises or {}).items():
             self.noise[s].copy_(n[0])
-        with nvtx_range("b200vton.slot_denoise_step"):
-            if use_graph:
-                if self._graph is None:
-                    self.capture()
-                self._graph.replay()
-            else:
-                self._launch_step()
-        return self.latents

@@ -15,7 +15,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 import torch
 
 from . import clip as _clip
-from .denoise import TryOnDenoiser, scheduler_kind
+from .denoise import TryOnDenoiser, check_guidance_rescale, scheduler_kind, variance_noise
 from .vae import VaeImageProcessor
 
 PipelineImageInput = Any
@@ -656,10 +656,8 @@ class StableDiffusionXLInpaintPipeline:
                           callback_on_step_end_tensor_inputs, padding_mask_crop)
         # the engine's fused step implements DDPM, DDIM, Euler and DPM-Solver++(2M): any other scheduler class raises
         # here, before any work, instead of being stepped with the wrong update
-        kind = scheduler_kind(self.scheduler)
-        if guidance_rescale > 0 and kind != "ddpm":
-            raise NotImplementedError(f"guidance_rescale with {type(self.scheduler).__name__}: the engine's guidance "
-                                      "rescale is fused with the DDPM step only")
+        scheduler_kind(self.scheduler)
+        check_guidance_rescale(self.scheduler, guidance_rescale)
         self._guidance_scale = guidance_scale
         self._guidance_rescale = guidance_rescale
         self._clip_skip = clip_skip
@@ -814,13 +812,7 @@ class StableDiffusionXLInpaintPipeline:
             for i, t in enumerate(timesteps):
                 if self.interrupt:
                     continue
-                # the variance noise the scheduler's own step would draw, in the same order (DDPM at t > 0, DDIM at
-                # eta > 0, Euler at every step), so the generator ends in the reference's state; Euler's draw is unused
-                step_noise = None
-                if den.step_draws[i]:
-                    step_noise = randn_tensor(latents.shape, generator=generator, device=device, dtype=latents.dtype)
-                    if not den.noise_applied:
-                        step_noise = None
+                step_noise = variance_noise(den, i, latents.shape, generator, device, latents.dtype)
                 latents = den.step(i, step_noise, use_graph=self.use_cuda_graph)
                 if callback_on_step_end is not None:
                     callback_kwargs = {k: locals()[k] for k in callback_on_step_end_tensor_inputs}

@@ -584,11 +584,16 @@ class DPMSolverMultistepScheduler(_FromConfig):
         return type("SchedulerOutput", (), dict(prev_sample=prev_sample))()
 
 
+def config_getter(config):
+    """get(key, default) on a scheduler config: a dict (diffusers' FrozenDict) or an object with attributes (or None)."""
+    return (lambda k, d=None: config.get(k, d)) if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+
+
 def solver_order_at(steps_taken, step_index, n_timesteps, config):
     """Order of DPMSolverMultistepScheduler.step at `step_index` of a schedule of `n_timesteps`, after `steps_taken`
     steps of this run: 1 for the run's first step, for solver_order 1, and for the last step of the schedule when
     euler_at_final is set or lower_order_final is set with fewer than 15 timesteps; 2 otherwise."""
-    get = (lambda k, d=None: config.get(k, d)) if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+    get = config_getter(config)
     final = step_index == n_timesteps - 1 and (get("euler_at_final", False)
                                                or (get("lower_order_final", True) and n_timesteps < 15))
     if get("solver_order", 2) == 1 or steps_taken < 1 or final:

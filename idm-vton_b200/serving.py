@@ -376,16 +376,15 @@ class ContinuousTryOnServer:
         active = [s for s, e in enumerate(self.slots) if e is not None]
         if not active:
             return {}
-        from .pipeline import randn_tensor
+        from .denoise import variance_noise
         den = self.den
         device = self.pipe._execution_device
         noises = {}
-        for s in active:                 # the variance noise the scheduler's own step would draw (pipeline order)
+        for s in active:
             e = self.slots[s]
-            if den.step_draws[e["step"]]:
-                n = randn_tensor((1, 4, *self.latent_size), generator=e["gen"], device=device, dtype=den.latents.dtype)
-                if den.noise_applied:
-                    noises[s] = n
+            n = variance_noise(den, e["step"], (1, 4, *self.latent_size), e["gen"], device, den.latents.dtype)
+            if n is not None:
+                noises[s] = n
         latents = den.step([None if e is None else e["step"] for e in self.slots], noises,
                            use_graph=use_graph and getattr(self.pipe, "use_cuda_graph", True))
         self.stats["steps"] += 1
