@@ -70,6 +70,9 @@ int cfg_ddpm_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, con
 int cfg_solver_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
                          void* x0_prev, const void* coef, int coef_stride, int kind, int do_cfg, void* out,
                          cudaStream_t stream);
+int cfg_mixed_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                        void* x0_prev, const void* coef, int coef_stride, const void* kinds, int do_cfg, void* out,
+                        cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
@@ -261,6 +264,12 @@ int b200vton_cfg_solver_step_rows(const void* eps, int ldc, int B, int C, int H,
                                   int do_cfg, void* out, void* stream) {
   return vton::cfg_solver_rows_impl(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, coef_stride, kind, do_cfg, out,
                                     S(stream));
+}
+int b200vton_cfg_step_mixed_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                 const void* noise, void* x0_prev, const void* coef, int coef_stride, const void* kinds,
+                                 int do_cfg, void* out, void* stream) {
+  return vton::cfg_mixed_rows_impl(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, coef_stride, kinds, do_cfg, out,
+                                   S(stream));
 }
 
 int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_channels, const void* image_min, int B,

@@ -267,6 +267,15 @@ int skinny_linear_impl(const void* x, int ldx, int M, int K, const void* W, long
 // ROWS (b200vton_cfg_ddpm_step_rows): coef is [B, coef_stride] and sample b reads row b, so every sample of the batch
 // can be at its own denoise step (continuous batching); coef_stride 0 is the single-row kernel.
 // ------------------------------------------------------------------------------------------------
+// The per-value pieces of the step kernels below, shared so that every kernel rounds at the same points.
+__device__ __forceinline__ float cfg_guided(float u, float t, float gs) { return round_h(u + round_h(gs * round_h(t - u))); }
+
+// DDPM update without its noise term: x0 = fp16(fp16(x - fp16(sb * g)) * inv_sa); prev = fp16(fp16(c0 x0) + fp16(c1 x)).
+__device__ __forceinline__ float ddpm_update(float x, float g, float sb, float inv_sa, float c0, float c1) {
+  const float x0 = round_h(round_h(x - round_h(sb * g)) * inv_sa);
+  return round_h(round_h(c0 * x0) + round_h(c1 * x));
+}
+
 template <bool ROWS>
 __global__ void cfg_ddpm_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents,
                                 const __half* noise, const float* coef, int coef_stride, int do_cfg, __half* out) {
@@ -282,13 +291,12 @@ __global__ void cfg_ddpm_kernel(const __half* eps, int ldc, int B, int C, int HW
   if (do_cfg) {
     const float u = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
     const float t = h2f(eps[(static_cast<long long>(b + B) * HW + px) * ldc + c]);
-    g = round_h(u + round_h(gs * round_h(t - u)));
+    g = cfg_guided(u, t, gs);
   } else {
     g = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
   }
   const float x = h2f(latents[i]);
-  const float x0 = round_h(round_h(x - round_h(sb * g)) * inv_sa);
-  float prev = round_h(round_h(c0 * x0) + round_h(c1 * x));
+  float prev = ddpm_update(x, g, sb, inv_sa, c0, c1);
   if (noise) prev = round_h(prev + round_h(sigma * h2f(noise[i])));
   out[i] = f2h(prev);
 }
@@ -354,11 +362,11 @@ __device__ __forceinline__ double cta_sum(double v, double* red) {
   return v;
 }
 
-__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_ddpm_kernel(
-    const __half* eps, int ldc, int B, int C, int HW, const __half* latents, const __half* noise, const float* coef,
-    __half* out) {
-  __shared__ double red[kRescaleThreads / 32];
-  const int b = blockIdx.x;
+// The rescaled step of sample b by one CTA of kRescaleThreads threads (cfg_rescale_ddpm_kernel; the DDPM rows with
+// phi > 0 of cfg_mixed_kernel). coef: the sample's row.
+__device__ __forceinline__ void rescale_ddpm_sample(const __half* eps, int ldc, int B, int C, int HW, int b,
+                                                    const __half* latents, const __half* noise, const float* coef,
+                                                    __half* out, double* red) {
   const float gs = coef[0], sb = coef[1], inv_sa = coef[2], c0 = coef[3], c1 = coef[4], sigma = coef[5], phi = coef[6];
   const __half* eu = eps + static_cast<long long>(b) * HW * ldc;         // uncond rows of sample b
   const __half* et = eps + static_cast<long long>(b + B) * HW * ldc;     // cond rows of sample b
@@ -367,7 +375,7 @@ __global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_ddpm_kernel(
   auto cfg = [&](long long off, float& t) {
     const float u = h2f(eu[off]);
     t = h2f(et[off]);
-    return round_h(u + round_h(gs * round_h(t - u)));
+    return cfg_guided(u, t, gs);
   };
   // pass 1: means (NHWC order: consecutive threads read consecutive channels / pixels)
   double st = 0.0, sg = 0.0;
@@ -403,11 +411,17 @@ __global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_ddpm_kernel(
     const float g = cfg(static_cast<long long>(px) * ldc + c, t);
     const float gr = round_h(round_h(phi * round_h(g * r)) + round_h((1.0f - phi) * g));
     const float x = h2f(latents[base + k]);
-    const float x0 = round_h(round_h(x - round_h(sb * gr)) * inv_sa);
-    float prev = round_h(round_h(c0 * x0) + round_h(c1 * x));
+    float prev = ddpm_update(x, gr, sb, inv_sa, c0, c1);
     if (noise) prev = round_h(prev + round_h(sigma * h2f(noise[base + k])));
     out[base + k] = f2h(prev);
   }
+}
+
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_ddpm_kernel(
+    const __half* eps, int ldc, int B, int C, int HW, const __half* latents, const __half* noise, const float* coef,
+    __half* out) {
+  __shared__ double red[kRescaleThreads / 32];
+  rescale_ddpm_sample(eps, ldc, B, C, HW, blockIdx.x, latents, noise, coef, out, red);
 }
 
 int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
@@ -444,6 +458,26 @@ int cfg_rescale_ddpm_impl(const void* eps, int ldc, int B, int C, int H, int W, 
 //          out = fp16((p x + fp16(q x0)) + fp16(fp32(q / 2) * fp16(k * fp16(x0 - x0_prev))));  x0_prev = x0
 // sigma_n * noise is added the same way by every kind when noise is not null (only DDIM with eta > 0 draws it).
 // ------------------------------------------------------------------------------------------------
+// The update of one value of kind KIND without its noise term; x0_prev: this value's DPM-Solver++ state (KIND 2 only).
+template <int KIND>
+__device__ __forceinline__ float solver_update(float x, float g, float s, float inv_a, float p, float q, float r, float k,
+                                               __half* x0_prev) {
+  if constexpr (KIND == 0) {
+    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
+    return round_h(round_h(q * x0) + round_h(r * g));
+  } else if constexpr (KIND == 1) {
+    const float x0 = __fsub_rn(x, round_h(s * g));
+    const float d = __fmul_rn(__fsub_rn(x, x0), inv_a);
+    return round_h(__fadd_rn(x, __fmul_rn(d, r)));
+  } else {
+    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
+    const float d1 = round_h(k * round_h(x0 - h2f(*x0_prev)));
+    const float prev = round_h(__fadd_rn(__fadd_rn(__fmul_rn(p, x), round_h(q * x0)), round_h(0.5f * q * d1)));
+    *x0_prev = f2h(x0);
+    return prev;
+  }
+}
+
 // ROWS (b200vton_cfg_solver_step_rows): coef is [B, coef_stride], sample b reads row b (coef_stride 0: one row for all).
 template <int KIND, bool ROWS>
 __global__ void cfg_solver_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents,
@@ -462,25 +496,12 @@ __global__ void cfg_solver_kernel(const __half* eps, int ldc, int B, int C, int 
   if (do_cfg) {
     const float u = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
     const float t = h2f(eps[(static_cast<long long>(b + B) * HW + px) * ldc + c]);
-    g = round_h(u + round_h(gs * round_h(t - u)));
+    g = cfg_guided(u, t, gs);
   } else {
     g = h2f(eps[(static_cast<long long>(b) * HW + px) * ldc + c]);
   }
   const float x = h2f(latents[i]);
-  float prev;
-  if constexpr (KIND == 0) {
-    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
-    prev = round_h(round_h(q * x0) + round_h(r * g));
-  } else if constexpr (KIND == 1) {
-    const float x0 = __fsub_rn(x, round_h(s * g));
-    const float d = __fmul_rn(__fsub_rn(x, x0), inv_a);
-    prev = round_h(__fadd_rn(x, __fmul_rn(d, r)));
-  } else {
-    const float x0 = round_h(round_h(x - round_h(s * g)) * inv_a);
-    const float d1 = round_h(k * round_h(x0 - h2f(x0_prev[i])));
-    prev = round_h(__fadd_rn(__fadd_rn(__fmul_rn(p, x), round_h(q * x0)), round_h(0.5f * q * d1)));
-    x0_prev[i] = f2h(x0);
-  }
+  float prev = solver_update<KIND>(x, g, s, inv_a, p, q, r, k, KIND == 2 ? x0_prev + i : nullptr);
   if (noise) prev = round_h(prev + round_h(sigma_n * h2f(noise[i])));
   out[i] = f2h(prev);
 }
@@ -527,6 +548,77 @@ int cfg_solver_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, c
                          cudaStream_t stream) {
   return launch_cfg_solver<true>(eps, ldc, B, C, H, W, latents, noise, x0_prev, coef, coef_stride, kind, do_cfg, out,
                                  stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Mixed-kind step (b200vton_cfg_step_mixed_rows): sample b takes the update of kinds[b] with coefficient row b, so one
+// launch steps a batch whose samples follow different schedulers (the sampling presets of continuous batching).
+//   0 DDIM, 1 Euler, 2 DPM-Solver++: cfg_solver_kernel<kind, true>, row {gs, s, inv_a, p, q, r, sigma_n, k};
+//   3 DDPM: cfg_ddpm_kernel<true>, row {gs, sb, inv_sa, c0, c1, sigma, phi, 0}; under CFG with phi > 0 the guidance
+//     rescale of cfg_rescale_ddpm_kernel, by the same CTA-wide reduction (so the same bits as that kernel on the sample).
+// noise is added on DDPM and DDIM rows only (Euler draws a noise it does not apply; DPM-Solver++ draws none); x0_prev is
+// read and written by DPM-Solver++ rows only. Grid (B, G): CTA (b, y) takes the values y * 1024 + k * G * 1024 of
+// sample b in NCHW order; a rescaled sample needs its whole CTA for the statistics, so it runs on y = 0 alone. Every
+// value is computed from its own inputs only, so the bits do not depend on G.
+// ------------------------------------------------------------------------------------------------
+constexpr int kMixedKindDdpm = 3;
+
+__global__ void __launch_bounds__(kRescaleThreads)
+cfg_mixed_kernel(const __half* eps, int ldc, int B, int C, int HW, const __half* latents, const __half* noise,
+                 __half* x0_prev, const float* coef, int coef_stride, const int* kinds, int do_cfg, __half* out) {
+  __shared__ double red[kRescaleThreads / 32];
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x;
+  const int kind = kinds[b];
+  coef += static_cast<long long>(b) * coef_stride;
+  if (kind == kMixedKindDdpm && do_cfg && coef[6] > 0.f) {
+    if (blockIdx.y == 0) rescale_ddpm_sample(eps, ldc, B, C, HW, b, latents, noise, coef, out, red);
+    return;
+  }
+  const float gs = coef[0], c1 = coef[1], c2 = coef[2], c3 = coef[3], c4 = coef[4], c5 = coef[5], c6 = coef[6],
+              c7 = coef[7];
+  const __half* eu = eps + static_cast<long long>(b) * HW * ldc;
+  const __half* et = eps + static_cast<long long>(b + B) * HW * ldc;
+  const int n = C * HW;
+  const long long base = static_cast<long long>(b) * n;
+  const bool noisy = noise && (kind == 0 || kind == kMixedKindDdpm);
+  const float sigma = kind == 0 ? c6 : c5;
+  for (int k = blockIdx.y * kRescaleThreads + threadIdx.x; k < n; k += gridDim.y * kRescaleThreads) {
+    const long long off = static_cast<long long>(k % HW) * ldc + k / HW;
+    const float g = do_cfg ? cfg_guided(h2f(eu[off]), h2f(et[off]), gs) : h2f(eu[off]);
+    const float x = h2f(latents[base + k]);
+    float prev;
+    if (kind == 0) prev = solver_update<0>(x, g, c1, c2, c3, c4, c5, c7, nullptr);
+    else if (kind == 1) prev = solver_update<1>(x, g, c1, c2, c3, c4, c5, c7, nullptr);
+    else if (kind == 2) prev = solver_update<2>(x, g, c1, c2, c3, c4, c5, c7, x0_prev + base + k);
+    else prev = ddpm_update(x, g, c1, c2, c3, c4);
+    if (noisy) prev = round_h(prev + round_h(sigma * h2f(noise[base + k])));
+    out[base + k] = f2h(prev);
+  }
+}
+
+int cfg_mixed_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
+                        void* x0_prev, const void* coef, int coef_stride, const void* kinds, int do_cfg, void* out,
+                        cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && C > 0 && C <= ldc && H > 0 && W > 0 && eps && latents && x0_prev && coef && kinds && out,
+                 "cfg_step_mixed_rows: bad arguments (eps, latents, x0_prev, coef, kinds and out are required)");
+  VTON_CHECK_ARG(coef_stride == 0 || coef_stride >= kSolverCoefs,
+                 "cfg_step_mixed_rows: coef_stride %d is neither 0 nor >= %d", coef_stride, kSolverCoefs);
+  VTON_CHECK_ARG(static_cast<long long>(C) * H * W < (1LL << 31), "cfg_step_mixed_rows: sample too large");
+  VTON_CHECK_ARG(aligned_to(eps, 2) && aligned_to(latents, 2) && aligned_to(noise, 2) && aligned_to(x0_prev, 2) &&
+                     aligned_to(out, 2) && aligned_to(coef, 4) && aligned_to(kinds, 4),
+                 "cfg_step_mixed_rows: fp16 operands must be 2-byte aligned, coef and kinds 4-byte aligned");
+  // enough CTAs to cover the SMs twice (two 1024-thread CTAs fit one SM), at most one per 1024 values of a sample
+  const int n = C * H * W;
+  const int G = std::max(1, std::min(cdiv(n, kRescaleThreads), cdiv(2 * num_sms(), B)));
+  VTON_CUDA(launch_kernel(cfg_mixed_kernel, dim3(B, G), dim3(kRescaleThreads), 0, stream,
+                          static_cast<const __half*>(eps), ldc, B, C, H * W, static_cast<const __half*>(latents),
+                          static_cast<const __half*>(noise), static_cast<__half*>(x0_prev),
+                          static_cast<const float*>(coef), coef_stride, static_cast<const int*>(kinds), do_cfg,
+                          static_cast<__half*>(out)));
+  count_launch();
+  return kOk;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -197,6 +197,9 @@ def ddpm_step_coefficients(scheduler, t):
     return float(b_t ** 0.5), float(inv_sa), float(c0), float(c1), float(sigma)
 
 
+MIXED_KIND_CODES = {"ddim": 0, "euler": 1, "dpmpp": 2, "ddpm": 3}     # kinds[b] of b200vton_cfg_step_mixed_rows
+
+
 def identity_step_row(kind):
     """The coefficient row of an idle slot of SlotDenoiser: the step returns its latents unchanged (zeros stay zeros),
     whatever the finite eps. DDPM {gs, sb, inv_sa, c0, c1, sigma, phi, 0}: x0 = 0, prev = 1 * x; DDIM and DPM-Solver++
@@ -344,6 +347,7 @@ class _CapturedStep:
     # Default: ON inside the graph, OFF for eager launches.
     PDL_IN_GRAPH = __import__("os").environ.get("B200VTON_PDL_GRAPH", "1") == "1"
     _graph = _graph_sig = None   # the captured step and the _signature it was captured at
+    kinds = None                 # per-sample kind codes of the mixed-kind step (SlotDenoiser.configure_presets)
 
     def _signature(self):
         """What a captured step bakes in: the kernel selection and the address, shape and dtype of every buffer the
@@ -352,12 +356,12 @@ class _CapturedStep:
         garment = (self.x_g, self.t_g, self.ctx_g) if gkv_pre is None else gkv_pre
         return (self.kind, self.rescale, self.do_cfg, gkv_pre is not None) + _describe(
             [self.latents, self.latents_next, self.noise, self.x0_prev, self.x_t, self.t_t, self.coef, self.scale,
-             self.aug, self.ctx_t, garment])
+             self.kinds, self.aug, self.ctx_t, garment])
 
     def _launch_step(self):
         """The launch sequence of one denoise step over the static buffers (graph-capturable)."""
         L = self.L
-        if self.kind == "euler":                                  # scale_model_input on the latent channels only
+        if self.kind in ("euler", "mixed"):                       # scale_model_input on the latent channels only
             scatter = L.nchw_to_nhwc_scaled_rows if self.ROWS else L.nchw_to_nhwc_scaled
             scatter(self.latents, self.x_t, self.scale, c_off=0)
         else:
@@ -370,7 +374,10 @@ class _CapturedStep:
         temb_t = self.tryon.time_embedding(self.t_t, self.Bt, self.aug)
         self.eps = self.tryon.forward(self.x_t, temb_t, self.ctx_t, gfeats=feats, gkv_pre=gkv_pre,
                                       n_persons=self.latents.shape[0] if self.do_cfg else 0)
-        if self.kind == "ddpm":
+        if self.kind == "mixed":                                  # one kind per sample
+            L.cfg_step_mixed_rows(self.eps, self.latents, self.noise, self.coef, self.kinds, self.x0_prev,
+                                  do_cfg=self.do_cfg, out=self.latents_next)
+        elif self.kind == "ddpm":
             step = L.cfg_ddpm_step_rows if self.ROWS else L.cfg_rescale_ddpm_step if self.rescale else L.cfg_ddpm_step
             step(self.eps, self.latents, self.noise, self.coef, do_cfg=self.do_cfg, out=self.latents_next)
         else:
@@ -385,7 +392,7 @@ class _CapturedStep:
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())
         keep = self.latents.clone()
-        keep_x0 = self.x0_prev.clone() if self.kind == "dpmpp" else None     # the warm-up step advances the state
+        keep_x0 = self.x0_prev.clone() if self.x0_prev is not None else None  # the warm-up step advances the state
         with torch.cuda.stream(s):
             self._launch_step()
         torch.cuda.current_stream().wait_stream(s)
@@ -638,12 +645,17 @@ class SlotDenoiser(_CapturedStep):
         b200vton_attention_rows, and an idle slot reads row -1, the zero-K/V closed form (no K/V traffic, and no
         unwritten memory is ever read). The caller (ContinuousTryOnServer) decides which garment is in which page.
 
+    Sampling presets (configure_presets): the slots may follow different StepPlans (scheduler, step count, strength,
+    guidance scale, DDPM guidance rescale). Their rows share one table with a kind code per row, a slot names (plan,
+    step), and the step is the mixed-kind kernel after the scaled scatter; a slot's result is the bits the per-kind
+    kernels give it. In pool mode a page holds T_max rows and a plan of T steps uses its first T.
+
     Idle slots hold zeros and the identity coefficient row (identity_step_row); their outputs are ignored. No row of one
     slot enters another slot's result, so at a fixed S a request's result does not depend on which slot it runs in or on
     what the other slots hold."""
 
     ROWS = True
-    rescale = False              # refused by configure: the rescale kernel reads one coefficient row for the batch
+    rescale = False              # refused by configure (the rescale kernel reads one row); per row in configure_presets
 
     def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots, pages=None):
         self.tryon, self.garment = tryon, garment
@@ -658,10 +670,12 @@ class SlotDenoiser(_CapturedStep):
         self.pool = None
         self._key = None
         self.ctx_t = None
+        self.plans = self.kind_table = None         # configure_presets: the plans and the kind of every table row
 
     def _needs(self, kind):
-        names = ["b200vton_cfg_ddpm_step_rows" if kind == "ddpm" else "b200vton_cfg_solver_step_rows"]
-        if kind == "euler":
+        names = ["b200vton_cfg_step_mixed_rows" if kind == "mixed" else
+                 "b200vton_cfg_ddpm_step_rows" if kind == "ddpm" else "b200vton_cfg_solver_step_rows"]
+        if kind in ("euler", "mixed"):
             names.append("b200vton_nchw_to_nhwc_scaled_rows")
         if self.P is not None:
             names.append("b200vton_attention_rows")
@@ -680,18 +694,60 @@ class SlotDenoiser(_CapturedStep):
             if not self.L.has_symbol(name):
                 raise NotImplementedError(f"continuous batching needs {name}, which this library binding does not export")
         vars(self).update(plan.to(self.device)._asdict())                  # kind, coef_table, ..., T
+        self.plans = self.kind_table = None
+        self.T_page = self.T
+        self._allocate(h, w, do_cfg)
+        self.gather([None] * self.S)
+
+    def configure_presets(self, plans, h, w, do_cfg=True):
+        """Per-step tables of several runs at once (sampling presets), stepped together by the mixed-kind step kernel
+        (b200vton_cfg_step_mixed_rows): plans is a list of StepPlan (step_plan, DDPM rows may carry a guidance
+        rescale). Their rows are concatenated into one coefficient / timestep / input-scale table (scale 1 for the
+        kinds that do not scale their input, which the scaled scatter applies exactly) with one kind code per row
+        (MIXED_KIND_CODES) and one identity row at the end for idle slots; plan j's step i is row base[j] + i. In pool
+        mode a page holds T_max = the largest T of the plans rows. Raises before any launch when the library lacks an
+        entry point this needs."""
+        plans = list(plans)
+        if not plans:
+            raise ValueError("configure_presets needs at least one StepPlan")
+        for name in self._needs("mixed"):
+            if not self.L.has_symbol(name):
+                raise NotImplementedError(f"sampling presets need {name}, which this library binding does not export")
+        f32 = torch.float32
+        idle = plans[0].kind
+        self.base, n = [], 0
+        for p in plans:
+            self.base.append(n)
+            n += p.T
+        self.idle = n
+        coef = torch.cat([p.coef_table[:p.T].cpu() for p in plans] + [torch.tensor([identity_step_row(idle)], dtype=f32)])
+        t = torch.cat([p.t_table[:p.T].cpu() for p in plans] + [torch.zeros(1, dtype=f32)])
+        scale = torch.cat([torch.ones(p.T, dtype=f32) if p.scale_table is None else p.scale_table[:p.T].cpu()
+                           for p in plans] + [torch.ones(1, dtype=f32)])
+        kinds = [MIXED_KIND_CODES[p.kind] for p in plans for _ in range(p.T)] + [MIXED_KIND_CODES[idle]]
+        dev = self.device
+        self.coef_table, self.t_table, self.scale_table = coef.to(dev), t.to(dev), scale.to(dev)
+        self.kind_table = torch.tensor(kinds, dtype=torch.int32).to(dev)
+        self.plans = plans
+        self.kind, self.T, self.step_draws, self.noise_applied = "mixed", None, None, None
+        self.T_page = max(p.T for p in plans)
+        self._allocate(h, w, do_cfg)
+        self.gather([None] * self.S)
+
+    def _allocate(self, h, w, do_cfg):
+        """The static buffers of a person latent size h x w (the garment has the same size), kept while the key holds."""
         dev, f16, f32 = self.device, torch.float16, torch.float32
         self.do_cfg, self.h, self.w = bool(do_cfg), h, w
         S = self.S
         self.Bt = 2 * S if do_cfg else S
-        key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T))
+        key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T_page))
         if key != self._key:
             self._key = key
             self.ctx_t = self.ctx_g = self.aug = None
             self.latents = torch.zeros((S, 4, h, w), dtype=f16, device=dev)
             self.latents_next = torch.zeros_like(self.latents)
             self.noise = torch.zeros_like(self.latents)
-            self.x0_prev = torch.zeros_like(self.latents) if self.kind == "dpmpp" else None
+            self.x0_prev = torch.zeros_like(self.latents) if self.kind in ("dpmpp", "mixed") else None
             self.x_t = torch.zeros((self.Bt, h, w, CIN_PAD), dtype=f16, device=dev)
             if self.P is None:
                 self.x_g = torch.zeros((S, h, w, CIN_PAD), dtype=f16, device=dev)
@@ -700,19 +756,30 @@ class SlotDenoiser(_CapturedStep):
                 # allocated once (the old pool is released first); every page is written by fill_page before a slot's
                 # row names it
                 self.x_g = self.t_g = self.pool = None
-                self.pool = [torch.empty((self.P * self.T, ng, 2 * b.c), dtype=f16, device=dev)
+                self.pool = [torch.empty((self.P * self.T_page, ng, 2 * b.c), dtype=f16, device=dev)
                              for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, h, w))]
                 self.rows = torch.full((S,), -1, dtype=torch.int32, device=dev)
                 self.page = [None] * S
             self.t_t = torch.zeros(self.Bt, dtype=f32, device=dev)
             self.coef = torch.zeros((S, 8), dtype=f32, device=dev)
             self.scale = torch.ones(S, dtype=f32, device=dev)
-        self.gather([None] * S)
+            self.kinds = torch.zeros(S, dtype=torch.int32, device=dev) if self.kind == "mixed" else None
 
     def gather(self, steps):
-        """steps: per slot, the step index of its request or None (idle). Copies row steps[s] (row T when idle) of the
-        tables into the graph's static t / coef / scale buffers (t at rows s and S + s of the try-on batch)."""
-        idx = torch.tensor([self.T if i is None else int(i) for i in steps], dtype=torch.long).to(self.device)
+        """steps: per slot, the step index of its request or None (idle); after configure_presets, (plan index, step
+        index) or None. Copies the slot's row of the tables (the idle row when idle) into the graph's static t / coef /
+        scale / kind buffers (t at rows s and S + s of the try-on batch)."""
+        if self.plans is None:
+            step_of = list(steps)
+            rows = [self.T if i is None else int(i) for i in steps]
+        else:
+            step_of, rows = [], []
+            for s, e in enumerate(steps):
+                if e is not None and not (0 <= e[0] < len(self.plans) and 0 <= e[1] < self.plans[e[0]].T):
+                    raise ValueError(f"slot {s}: (plan, step) {tuple(e)} outside the configured plans")
+                step_of.append(None if e is None else int(e[1]))
+                rows.append(self.idle if e is None else self.base[e[0]] + int(e[1]))
+        idx = torch.tensor(rows, dtype=torch.long).to(self.device)
         torch.index_select(self.coef_table, 0, idx, out=self.coef)
         t = self.t_table.index_select(0, idx)
         if self.t_g is not None:
@@ -720,35 +787,48 @@ class SlotDenoiser(_CapturedStep):
         self.t_t.copy_(t.repeat(self.Bt // self.S))
         if self.scale_table is not None:
             torch.index_select(self.scale_table, 0, idx, out=self.scale)
+        if self.kind_table is not None:
+            torch.index_select(self.kind_table, 0, idx, out=self.kinds)
         if self.P is not None:
-            # pool mode: slot s reads row page(s) * T + step(s) of the pool, an idle slot row -1 (zero K/V)
+            # pool mode: slot s reads row page(s) * T_page + step(s) of the pool, an idle slot row -1 (zero K/V)
             rows = []
-            for s, i in enumerate(steps):
+            for s, i in enumerate(step_of):
                 if i is not None and self.page[s] is None:
                     raise ValueError(f"slot {s} is at step {i} but holds no garment K/V page")
-                rows.append(-1 if i is None else self.page[s] * self.T + int(i))
-            if any(not -1 <= r < self.P * self.T for r in rows):
-                raise ValueError(f"garment K/V rows {rows} outside [-1, {self.P * self.T})")
+                rows.append(-1 if i is None else self.page[s] * self.T_page + int(i))
+            if any(not -1 <= r < self.P * self.T_page for r in rows):
+                raise ValueError(f"garment K/V rows {rows} outside [-1, {self.P * self.T_page})")
             self.rows.copy_(torch.tensor(rows, dtype=torch.int32))
 
-    def fill_page(self, p, cloth_latents, text_embeds_cloth):
+    def fill_page(self, p, cloth_latents, text_embeds_cloth, t_table=None):
         """Pool mode: writes the garment K/V of all T steps of one garment (cloth_latents [1,4,h,w], text_embeds_cloth
         [1,77,X]) into page p: its T garment-UNet passes at Bg = 1, chunked as TryOnDenoiser chunks them, so the page
-        holds the bits TryOnDenoiser's gkv_all holds for that garment alone. Runs eagerly (not in the step graph)."""
+        holds the bits TryOnDenoiser's gkv_all holds for that garment alone. Runs eagerly (not in the step graph).
+        t_table: after configure_presets, the timesteps of the plan the page is filled for (its first rows then hold
+        them; required), else the configured run's."""
         if self.P is None or self.pool is None:
             raise RuntimeError("SlotDenoiser.fill_page needs pool mode (pages=P) and configure() first")
         if not 0 <= p < self.P:
             raise ValueError(f"page {p} outside [0, {self.P})")
+        if t_table is None:
+            if self.plans is not None:
+                raise ValueError("fill_page after configure_presets needs the timesteps of the page's plan")
+            t_table, T = self.t_table, self.T
+        else:
+            t_table = t_table.to(self.device, torch.float32)
+            T = t_table.shape[0]
+            if not 0 < T <= self.T_page:
+                raise ValueError(f"{T} timesteps do not fit a page of {self.T_page} rows")
         if tuple(cloth_latents.shape[-2:]) != (self.h, self.w):
             raise ValueError(f"cloth_latents has spatial size {tuple(cloth_latents.shape[-2:])}, the server's latents "
                              f"{(self.h, self.w)}")
-        dev, f16, T = self.device, torch.float16, self.T
+        dev, f16, Tp = self.device, torch.float16, self.T_page
         with nvtx_range(f"b200vton.garment_page_fill[{p}]"):
             x_g = torch.zeros((1, self.h, self.w, CIN_PAD), dtype=f16, device=dev)
             self.L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), x_g, c_off=0)
             ctx_g = self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16))
-            hoisted_garment_kv(self.tryon, self.garment, x_g, ctx_g, self.t_table, 0, T, self.garment_chunk,
-                               [g[p * T:(p + 1) * T] for g in self.pool])
+            hoisted_garment_kv(self.tryon, self.garment, x_g, ctx_g, t_table, 0, T, self.garment_chunk,
+                               [g[p * Tp:p * Tp + T] for g in self.pool])
 
     def _rows(self, s):
         return (s, self.S + s) if self.do_cfg else (s,)

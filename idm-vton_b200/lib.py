@@ -48,7 +48,8 @@ SIGNATURES = {
 }
 
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
-# step kernels of the continuous-batching denoiser, the FP8 linears and the per-sample-row attention of its pool mode.
+# step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears and
+# the per-sample-row attention of its pool mode.
 # `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
@@ -58,6 +59,7 @@ OPTIONAL_SIGNATURES = {
     "b200vton_layernorm_e4m3": [_vp, _i64, _i, _i, _vp, _vp, _f, _vp, _i64, _vp, _i64, _vp, _vp],
     "b200vton_attention_rows": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp,
                                 _f, _i, _vp],
+    "b200vton_cfg_step_mixed_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp],
 }
 _present = set()
 
@@ -770,3 +772,23 @@ def nchw_to_nhwc_scaled_rows(src, dst, scale, c_off=0):
     rc = fn(_p(src), Bs, Cs, H, W, _p(dst), dst.shape[0], dst.shape[-1], c_off, _p(scale), _stream())
     _check(rc, "b200vton_nchw_to_nhwc_scaled_rows")
     return dst
+
+
+
+def cfg_step_mixed_rows(eps, latents, noise, coef, kinds, x0_prev, do_cfg=True, out=None):
+    """One step of a batch whose samples follow different schedulers: sample b takes kind kinds[b] (0 DDIM, 1 Euler, 2 DPM-Solver++, 3 DDPM) with
+    coefficient row b of coef [B, 8] fp32 (DDPM rows {gs, sb, inv_sa, c0, c1, sigma, phi, 0}, the others as
+    cfg_solver_step). noise enters DDPM and DDIM rows only; x0_prev [B,C,H,W] fp16 is required and only DPM-Solver++
+    rows read and rewrite it. kinds: contiguous CUDA int32 tensor of B entries."""
+    fn = _optional("b200vton_cfg_step_mixed_rows")
+    B, C, H, W = latents.shape
+    stride = _coef_rows(coef, B, "cfg_step_mixed_rows")
+    if kinds.dtype != torch.int32 or not kinds.is_cuda or not kinds.is_contiguous() or kinds.numel() != B:
+        raise ValueError(f"cfg_step_mixed_rows: kinds must be a contiguous CUDA int32 tensor of B = {B} entries, got "
+                         f"{kinds.dtype} {tuple(kinds.shape)} on {kinds.device}")
+    if out is None:
+        out = torch.empty_like(latents)
+    rc = fn(_p(eps), eps.shape[-1], B, C, H, W, _p(latents), _p(noise), _p(x0_prev), _p(coef), stride, _p(kinds),
+            int(do_cfg), _p(out), _stream())
+    _check(rc, "b200vton_cfg_step_mixed_rows")
+    return out

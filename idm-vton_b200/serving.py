@@ -13,6 +13,8 @@ why the cache is a property of this front-end and not of the pipeline (off unles
 Single-threaded by design, like the reference pipeline (one CUDA stream, one denoiser / graph per process).
 """
 import collections
+import contextlib
+import copy
 import dataclasses
 from typing import Any, Hashable, Optional
 
@@ -38,6 +40,59 @@ class TryOnRequest:
     text_embeds_cloth: Optional[torch.Tensor] = None  # [77,2048]
     ticket: Any = None
     seed: Optional[int] = None          # ContinuousTryOnServer: this request's generator (TryOnServer ignores it)
+    sampling: Optional[Hashable] = None  # the name of the server's SamplingPreset; None: the server's default preset
+
+
+@dataclasses.dataclass
+class SamplingPreset:
+    """How a request is denoised: the pipeline's `__call__` arguments of the same names. scheduler: a diffusers-style
+    scheduler object (None: the pipeline's); the server steps a private copy of it."""
+    scheduler: Any = None
+    num_inference_steps: int = 30
+    guidance_scale: float = 2.0
+    strength: float = 1.0
+    eta: float = 0.0
+    guidance_rescale: float = 0.0
+
+
+def _check_presets(presets, default_preset):
+    """(presets, default name) of a server's `presets` / `default_preset` arguments: a non-empty dict of SamplingPreset;
+    the default may be omitted when there is one preset."""
+    presets = dict(presets)
+    if not presets or not all(isinstance(p, SamplingPreset) for p in presets.values()):
+        raise ValueError("presets must be a non-empty dict of name -> SamplingPreset")
+    if default_preset is None and len(presets) == 1:
+        default_preset = next(iter(presets))
+    if default_preset not in presets:
+        raise ValueError(f"default_preset {default_preset!r} is not one of the presets {list(presets)}")
+    return presets, default_preset
+
+
+def _preset_name(server, req):
+    name = server.default_preset if req.sampling is None else req.sampling
+    if name not in server.presets:
+        raise ValueError(f"request names sampling preset {req.sampling!r}; the server has {list(server.presets)}")
+    return name
+
+
+def _private(scheduler):
+    """A copy of `scheduler` whose set_timesteps leaves the original as it was: set_timesteps rebinds the attributes it
+    sets, and the shared config and training tables are only read."""
+    return copy.copy(scheduler)
+
+
+@contextlib.contextmanager
+def _scheduler_installed(pipe, scheduler):
+    """pipe.scheduler = scheduler for the block (None: the pipeline's own), restored afterwards."""
+    if scheduler is None:
+        yield
+        return
+    old = pipe.scheduler
+    pipe.scheduler = scheduler
+    try:
+        yield
+    finally:
+        pipe.scheduler = old
 
 
 def _encode_garment(pipe, src, seed, device, dtype):
@@ -68,15 +123,26 @@ def _seeded_global_rng(device, seed):
 
 
 class TryOnServer:
+    """Batch mode: requests that wear the same garment and use the same sampling preset run as one pipeline call.
+    presets: {name: SamplingPreset} (a request picks one by `sampling`; default_preset when it names none); each batch
+    calls the pipeline with its preset's arguments, its scheduler (a private copy) installed for the call. None: one
+    preset from num_inference_steps and guidance_scale with the pipeline's scheduler."""
+
     def __init__(self, pipe, height=1024, width=768, num_inference_steps=30, guidance_scale=2.0, max_batch=8, seed=None,
-                 garment_cache_bytes=40 << 30, output_type="pt"):
+                 garment_cache_bytes=40 << 30, output_type="pt", presets=None, default_preset=None):
         self.pipe = pipe
         self.height, self.width = height, width
         self.num_inference_steps, self.guidance_scale = num_inference_steps, guidance_scale
         self.max_batch = max_batch
         self.seed = seed
         self.output_type = output_type
-        self.queue = collections.OrderedDict()      # garment_id -> deque of requests (arrival order inside a garment)
+        if presets is None:
+            self.presets, self.default_preset = {None: None}, None       # built from the attributes at each batch
+        else:
+            self.presets, self.default_preset = _check_presets(presets, default_preset)
+        self._schedulers = {n: None if p is None or p.scheduler is None else _private(p.scheduler)
+                            for n, p in self.presets.items()}
+        self.queue = collections.OrderedDict()      # (garment_id, preset) -> deque of requests (arrival order)
         self.garments = {}                          # garment_id -> dict(latents, ip_adapter_image, text_embeds_cloth)
         self._next_ticket = 0
         self.stats = collections.Counter()
@@ -85,25 +151,30 @@ class TryOnServer:
 
     # ---------------------------------------------------------------------------------------------
     def submit(self, req: TryOnRequest):
-        if req.garment_id not in self.garments and req.garment_id not in self.queue and \
+        name = _preset_name(self, req)
+        if req.garment_id not in self.garments and all(g != req.garment_id for g, _ in self.queue) and \
                 (req.cloth is None or req.ip_adapter_image is None or req.text_embeds_cloth is None):
             raise ValueError(f"garment {req.garment_id!r} is new: cloth, ip_adapter_image and text_embeds_cloth are required")
         req.ticket = self._next_ticket
         self._next_ticket += 1
-        self.queue.setdefault(req.garment_id, collections.deque()).append(req)
+        self.queue.setdefault((req.garment_id, name), collections.deque()).append(req)
         return req.ticket
 
     def pending(self):
         return sum(len(q) for q in self.queue.values())
 
     def _next_batch(self):
-        """Oldest waiting request decides the garment; up to max_batch requests of that garment go together."""
-        gid = min(self.queue, key=lambda g: self.queue[g][0].ticket)
-        q = self.queue[gid]
+        """Oldest waiting request decides the garment and the preset; up to max_batch requests of both go together."""
+        key = min(self.queue, key=lambda k: self.queue[k][0].ticket)
+        q = self.queue[key]
         batch = [q.popleft() for _ in range(min(self.max_batch, len(q)))]
         if not q:
-            del self.queue[gid]
-        return gid, batch
+            del self.queue[key]
+        return key, batch
+
+    def _preset(self, name):
+        p = self.presets[name]
+        return SamplingPreset(None, self.num_inference_steps, self.guidance_scale) if p is None else p
 
     def _garment(self, gid, batch, device, dtype):
         g = self.garments.get(gid)
@@ -118,24 +189,27 @@ class TryOnServer:
         """Runs ONE batch; returns {ticket: image}."""
         if not self.queue:
             return {}
-        gid, batch = self._next_batch()
+        (gid, name), batch = self._next_batch()
+        preset = self._preset(name)
         pipe = self.pipe
         device = pipe._execution_device
         dtype = pipe.unet.dtype
         gen = torch.Generator(device).manual_seed(self.seed) if self.seed is not None else None
         g = self._garment(gid, batch, device, dtype)
         stack = lambda name, dt=None: torch.stack([getattr(r, name) for r in batch]).to(device=device, dtype=dt)  # noqa: E731
+        # eta and guidance_rescale are passed only when a preset sets them (the pipeline's defaults otherwise)
+        extra = {k: getattr(preset, k) for k in ("eta", "guidance_rescale") if getattr(preset, k)}
         # the pose latents' sample comes from the global generator: seeded around the call (_seeded_global_rng), so a
         # seeded server is reproducible
-        with _seeded_global_rng(device, self.seed):
+        with _scheduler_installed(pipe, self._schedulers[name]), _seeded_global_rng(device, self.seed):
             images = pipe(prompt_embeds=stack("prompt_embeds", dtype), negative_prompt_embeds=stack("negative_prompt_embeds", dtype),
                           pooled_prompt_embeds=stack("pooled_prompt_embeds", dtype),
                           negative_pooled_prompt_embeds=stack("negative_pooled_prompt_embeds", dtype),
-                          num_inference_steps=self.num_inference_steps, generator=gen, strength=1.0,
+                          num_inference_steps=preset.num_inference_steps, generator=gen, strength=preset.strength,
                           pose_img=stack("pose_img", dtype), text_embeds_cloth=g["text_embeds_cloth"], cloth=g["latents"],
                           mask_image=stack("mask_image"), image=stack("image"), height=self.height, width=self.width,
-                          ip_adapter_image=g["ip_adapter_image"], guidance_scale=self.guidance_scale,
-                          output_type=self.output_type, garment_keys=[gid])[0]
+                          ip_adapter_image=g["ip_adapter_image"], guidance_scale=preset.guidance_scale,
+                          output_type=self.output_type, garment_keys=[gid], **extra)[0]
         self.stats["batches"] += 1
         self.stats["images"] += len(batch)
         return {r.ticket: images[i] for i, r in enumerate(batch)}
@@ -156,9 +230,16 @@ class ContinuousTryOnServer:
     the requests that finished (one decode for all of them) and frees their slots. A request therefore waits for a free
     slot, not for a whole batch, and a batch that is not full fills up at the next step.
 
-    One scheduler (the pipeline's), one `num_inference_steps` and one guidance scale for every request, and one person
-    size (height x width); the garment must have the same latent size. Garments are VAE-encoded once per garment_id
-    exactly as TryOnServer does.
+    One person size (height x width); the garment must have the same latent size. Garments are VAE-encoded once per
+    garment_id exactly as TryOnServer does.
+
+    Sampling presets: presets=None runs every request with the pipeline's scheduler, num_inference_steps, guidance_scale
+    and eta at strength 1. presets={name: SamplingPreset} lets each request pick one by `sampling` (default_preset when
+    it names none): its own scheduler (a private copy per preset: one preset's set_timesteps touches no other preset
+    and not pipe.scheduler), step count, strength, guidance scale, eta and, with DDPM, guidance rescale. Every preset's
+    plan is built at the first step. One preset without guidance rescale runs the per-kind step kernels; two or more,
+    or guidance rescale, run SlotDenoiser.configure_presets and the mixed-kind step kernel, where each request gets the
+    bits it gets from a one-preset server. A request retires after its own preset's number of steps.
 
     Garment work, two modes:
       * garment_kv_bytes=None (default): the garment UNet runs inside every step at batch `slots` (no hoisting and no
@@ -178,12 +259,16 @@ class ContinuousTryOnServer:
     and neighbours (at a fixed number of slots): its final latents always, its image when it finishes at a step of its
     own (requests finishing at the same step share one VAE decode).
     `eta`: DDIM's eta, as the pipeline's `__call__` takes it (0 = deterministic DDIM, 1 = DDPM-like variance).
-    Refused: guidance_rescale (not a parameter here), schedulers other than DDPM / DDIM / Euler / DPM-Solver++, and a
-    library without the per-slot step kernels or, in pool mode, without b200vton_attention_rows (NotImplementedError
-    naming the symbol, before any launch)."""
+    Pool mode with presets: a page holds T_max (the largest step count of the presets) steps, and pages are keyed by
+    (garment_id, the preset's timesteps), so presets with the same timesteps share a garment's page.
+    Refused, before any launch: guidance_rescale without presets (not a parameter here) and with a scheduler other
+    than DDPM (NotImplementedError); presets with guidance_scale <= 1 beside presets with CFG (ValueError); schedulers
+    other than DDPM / DDIM / Euler / DPM-Solver++; a library without the per-slot step kernels, the mixed-kind step
+    kernel (b200vton_cfg_step_mixed_rows) when presets need it, or, in pool mode, b200vton_attention_rows
+    (NotImplementedError naming the symbol). An unknown preset name is refused at submit (ValueError)."""
 
     def __init__(self, pipe, height=1024, width=768, slots=4, num_inference_steps=30, guidance_scale=2.0, seed=None,
-                 output_type="pt", eta=0.0, garment_kv_bytes=None):
+                 output_type="pt", eta=0.0, garment_kv_bytes=None, presets=None, default_preset=None):
         self.pipe = pipe
         self.height, self.width = height, width
         self.S = int(slots)
@@ -192,6 +277,12 @@ class ContinuousTryOnServer:
         self.output_type = output_type
         self.eta = float(eta)                        # DDIM's eta (the pipeline's `eta`; other schedulers ignore it)
         self.guidance_rescale = 0.0
+        if presets is None:
+            self.presets, self.default_preset = {None: None}, None       # built from the attributes at configure
+        else:
+            self.presets, self.default_preset = _check_presets(presets, default_preset)
+        # two or more presets, or guidance rescale: the mixed-kind step
+        self.mixed = len(self.presets) > 1 or any(p is not None and p.guidance_rescale > 0 for p in self.presets.values())
         vsf = pipe.vae_scale_factor
         self.latent_size = (height // vsf, width // vsf)
         self.waiting = collections.deque()
@@ -208,6 +299,7 @@ class ContinuousTryOnServer:
 
     # ---------------------------------------------------------------------------------------------
     def submit(self, req: TryOnRequest):
+        _preset_name(self, req)
         known = req.garment_id in self.garments or any(r.garment_id == req.garment_id for r in self.waiting) or any(
             e is not None and e["req"].garment_id == req.garment_id for e in self.slots)
         if not known:
@@ -233,9 +325,12 @@ class ContinuousTryOnServer:
         return SlotDenoiser(self.pipe.unet.engine(), self.pipe.unet_encoder.engine(), self.S, pages=pages)
 
     def page_bytes(self, T=None):
-        """Pool mode: bytes of one garment's page, the hoisted K/V of all T steps at Bg = 1 (from the shapes)."""
+        """Pool mode: bytes of one garment's page, the hoisted K/V of all T steps at Bg = 1 (from the shapes). T defaults
+        to the step count of the run, or with presets to the largest one after strength (T_max)."""
         from .denoise import garment_kv_bytes_per_step
-        T = self.num_inference_steps if T is None else T
+        if T is None:
+            T = max(self.num_inference_steps if p is None else
+                    min(int(p.num_inference_steps * p.strength), p.num_inference_steps) for p in self.presets.values())
         return T * garment_kv_bytes_per_step(self.pipe.unet.engine(), *self.latent_size)
 
     def _pages(self, T):
@@ -253,15 +348,38 @@ class ContinuousTryOnServer:
         self.pins.clear()
         self.free_pages = list(range(P))
 
-    def _configure(self):
-        """Timesteps and per-step tables of the run (the pipeline's own timestep selection at strength 1); checks every
-        refusal before the first launch."""
+    def _preset(self, name):
+        p = self.presets[name]
+        return SamplingPreset(None, self.num_inference_steps, self.guidance_scale, 1.0, self.eta) if p is None else p
+
+    def _run_timesteps(self, name):
+        """The pipeline's own timestep selection for preset `name` (its scheduler installed: retrieve_timesteps, then
+        get_timesteps at the preset's strength)."""
         from .pipeline import retrieve_timesteps
+        pipe, p = self.pipe, self._preset(name)
+        with _scheduler_installed(pipe, self._schedulers[name]):
+            timesteps, n = retrieve_timesteps(pipe.scheduler, p.num_inference_steps, pipe._execution_device)
+            timesteps, n = pipe.get_timesteps(n, p.strength, pipe._execution_device)
+        if n < 1:
+            raise ValueError(f"sampling preset {name!r}: strength {p.strength} at {p.num_inference_steps} steps leaves "
+                             f"{n} steps")
+        return timesteps
+
+    def _configure(self):
+        """Timesteps and per-step tables of every preset (the pipeline's own timestep selection); checks every refusal
+        before the first launch."""
         pipe = self.pipe
-        pipe._guidance_scale = self.guidance_scale
-        timesteps, n = retrieve_timesteps(pipe.scheduler, self.num_inference_steps, pipe._execution_device)
-        timesteps, n = pipe.get_timesteps(n, 1.0, pipe._execution_device)
+        # private schedulers (presets given; the pipeline's own without presets)
+        self._schedulers = {n: None if p is None else _private(pipe.scheduler if p.scheduler is None else p.scheduler)
+                            for n, p in self.presets.items()}
+        if self.mixed:
+            return self._configure_presets()
+        name = next(iter(self.presets))
+        p = self._preset(name)
+        pipe._guidance_scale = p.guidance_scale
+        timesteps = self._run_timesteps(name)
         self.timesteps = timesteps
+        self._timesteps = {name: timesteps}
         if self.den is None:
             if self.garment_kv_bytes is None:
                 self.den = self._make_denoiser()
@@ -269,9 +387,39 @@ class ContinuousTryOnServer:
                 P = self._pages(len(timesteps))
                 self.den = self._make_denoiser(pages=P)
                 self._reset_pages(P)
-        self.den.configure(pipe.scheduler, timesteps, *self.latent_size, guidance_scale=self.guidance_scale,
-                           do_cfg=pipe.do_classifier_free_guidance, eta=self.eta, guidance_rescale=self.guidance_rescale)
+        self.den.configure(self._schedulers[name] or pipe.scheduler, timesteps, *self.latent_size,
+                           guidance_scale=p.guidance_scale, do_cfg=pipe.do_classifier_free_guidance, eta=p.eta,
+                           guidance_rescale=self.guidance_rescale)
         self.T = self.den.T
+        self._configured = True
+
+    def _configure_presets(self):
+        """The mixed-kind path: one StepPlan per preset, refusals first."""
+        from .denoise import check_guidance_rescale, scheduler_kind, step_plan
+        pipe = self.pipe
+        for name, p in self.presets.items():
+            scheduler_kind(self._schedulers[name])
+            check_guidance_rescale(self._schedulers[name], p.guidance_rescale)
+        if len({p.guidance_scale > 1 for p in self.presets.values()}) > 1:
+            raise ValueError("sampling presets with guidance_scale <= 1 (no classifier-free guidance) cannot share a "
+                             "server with presets that use it: " +
+                             ", ".join(f"{n!r}: {p.guidance_scale}" for n, p in self.presets.items()))
+        pipe._guidance_scale = self.presets[self.default_preset].guidance_scale
+        do_cfg = pipe.do_classifier_free_guidance
+        self._timesteps = {n: self._run_timesteps(n) for n in self.presets}
+        self._plan_index = {n: j for j, n in enumerate(self.presets)}
+        self.plans = [step_plan(self._schedulers[n], self._timesteps[n], p.guidance_scale,
+                                p.guidance_rescale if do_cfg else 0.0, p.eta) for n, p in self.presets.items()]
+        T_max = max(plan.T for plan in self.plans)
+        if self.den is None:
+            if self.garment_kv_bytes is None:
+                self.den = self._make_denoiser()
+            else:
+                P = self._pages(T_max)
+                self.den = self._make_denoiser(pages=P)
+                self._reset_pages(P)
+        self.den.configure_presets(self.plans, *self.latent_size, do_cfg=do_cfg)
+        self.T = T_max
         self._configured = True
 
     def _garment(self, req, device, dtype):
@@ -287,9 +435,15 @@ class ContinuousTryOnServer:
         return g
 
     def _prepare_request(self, req, gen):
-        """The pipeline's own preparation of one person (batch 1, strength 1): pre-processing, initial latents, mask and
-        masked-image latents, pose latents, prompt and added-condition embeddings — drawing from `gen` in the
-        pipeline's order. Returns the keyword arguments of SlotDenoiser.admit except the garment's."""
+        """The pipeline's own preparation of one person (batch 1, the request's preset and its scheduler installed):
+        pre-processing, initial latents (with strength < 1 the image's VAE sample, then the noise, added to it at the
+        first timestep), mask and masked-image latents, pose latents, prompt and added-condition embeddings — drawing
+        from `gen` in the pipeline's order. Returns the keyword arguments of SlotDenoiser.admit except the garment's."""
+        name = _preset_name(self, req)
+        with _scheduler_installed(self.pipe, self._schedulers[name]):
+            return self._prepare_with(req, gen, self._preset(name).strength, self._timesteps[name])
+
+    def _prepare_with(self, req, gen, strength, timesteps):
         pipe = self.pipe
         device, dtype = pipe._execution_device, pipe.unet.dtype
         do_cfg = pipe.do_classifier_free_guidance
@@ -303,7 +457,8 @@ class ContinuousTryOnServer:
         init_image, mask, masked_image, mask_latent = pipe._preprocess_image_mask(
             req.image[None].to(device=device), req.mask_image[None].to(device=device), None, H, W)
         latents, = pipe.prepare_latents(1, pipe.vae.config.latent_channels, H, W, pe.dtype, device, gen, None,
-                                        image=init_image, timestep=self.timesteps[:1], is_strength_max=True)  # draw 1
+                                        image=init_image, timestep=timesteps[:1],
+                                        is_strength_max=strength == 1.0)                                     # draw 1
         mask, masked_lat = pipe.prepare_mask_latents(mask, masked_image, 1, H, W, pe.dtype, device, gen, do_cfg,
                                                      _mask_latent=mask_latent)                               # draw 2
         with _seeded_global_rng(device, self._seed(req)):
@@ -338,18 +493,25 @@ class ContinuousTryOnServer:
             seed = self._seed(req)
             gen = torch.Generator(device).manual_seed(seed) if seed is not None else None
             prep = self._prepare_request(req, gen)
-            page = None if self.garment_kv_bytes is None else self._pin_page(req.garment_id, g)
+            if self.mixed:             # the slot runs plan j; the garment's page is keyed by that plan's timesteps
+                j = self._plan_index[_preset_name(self, req)]
+                T, t_table = self.plans[j].T, self.plans[j].t_table[:self.plans[j].T]
+                key = (req.garment_id, tuple(float(t) for t in t_table))
+            else:
+                j, T, t_table, key = None, self.T, None, req.garment_id
+            page = None if self.garment_kv_bytes is None else self._pin_page(key, g, t_table)
             self.den.admit(s, cloth_latents=g["latents"], image_embeds=g["image_embeds"],
                            text_embeds_cloth=g["text_embeds_cloth"], page=page, **prep)
-            self.slots[s] = dict(req=req, gen=gen, step=0, page=page)
+            self.slots[s] = dict(req=req, gen=gen, step=0, page=page, plan=j, T=T)
             self.stats["admitted"] += 1
 
-    def _pin_page(self, gid, g):
-        """Pool mode: the page holding garment `gid`, pinned for one more slot. A miss fills a free page, else the least
-        recently admitted unpinned one (one exists: a free slot means at most slots - 1 pinned pages, and P >= slots)."""
-        p = self.page_of.get(gid)
+    def _pin_page(self, key, g, t_table=None):
+        """Pool mode: the page holding `key` (the garment id; with the mixed-kind step, (garment id, the plan's
+        timesteps t_table)), pinned for one more slot. A miss fills a free page, else the least recently admitted
+        unpinned one (one exists: a free slot means at most slots - 1 pinned pages, and P >= slots)."""
+        p = self.page_of.get(key)
         if p is not None:
-            self.page_of.move_to_end(gid)
+            self.page_of.move_to_end(key)
             self.stats["garment_page_hits"] += 1
         else:
             if self.free_pages:
@@ -358,8 +520,8 @@ class ContinuousTryOnServer:
                 victim = next(k for k, q in self.page_of.items() if self.pins[q] == 0)
                 p = self.page_of.pop(victim)
                 self.stats["garment_page_evictions"] += 1
-            self.den.fill_page(p, g["latents"], g["text_embeds_cloth"])
-            self.page_of[gid] = p
+            self.den.fill_page(p, g["latents"], g["text_embeds_cloth"], *(() if t_table is None else (t_table,)))
+            self.page_of[key] = p
             self.stats["garment_page_fills"] += 1
         self.pins[p] += 1
         return p
@@ -382,17 +544,18 @@ class ContinuousTryOnServer:
         noises = {}
         for s in active:
             e = self.slots[s]
-            n = variance_noise(den, e["step"], (1, 4, *self.latent_size), e["gen"], device, den.latents.dtype)
+            plan = den if e["plan"] is None else self.plans[e["plan"]]      # the draws of the slot's own run
+            n = variance_noise(plan, e["step"], (1, 4, *self.latent_size), e["gen"], device, den.latents.dtype)
             if n is not None:
                 noises[s] = n
-        latents = den.step([None if e is None else e["step"] for e in self.slots], noises,
-                           use_graph=use_graph and getattr(self.pipe, "use_cuda_graph", True))
+        steps = [None if e is None else e["step"] if e["plan"] is None else (e["plan"], e["step"]) for e in self.slots]
+        latents = den.step(steps, noises, use_graph=use_graph and getattr(self.pipe, "use_cuda_graph", True))
         self.stats["steps"] += 1
         self.stats["slot_steps"] += len(active)
         done = []
         for s in active:
             self.slots[s]["step"] += 1
-            if self.slots[s]["step"] == self.T:
+            if self.slots[s]["step"] == self.slots[s]["T"]:
                 done.append(s)
         if not done:
             self.last_latents = {}

@@ -267,6 +267,18 @@ int b200vton_cfg_solver_step_rows(const void* eps, int ldc, int B, int C, int H,
                                   const void* noise, void* x0_prev, const void* coef, int coef_stride, int kind,
                                   int do_cfg, void* out, void* stream);
 
+/* One step of a batch whose samples follow different schedulers (sampling presets of continuous batching). Same layout
+ * as b200vton_cfg_solver_step_rows, plus kinds: a device int32 array of B entries, read after the kernel's
+ * griddepcontrol.wait. Sample b takes kind kinds[b] with coefficient row b:
+ *   0 DDIM, 1 Euler, 2 DPM-Solver++ (row {gs, s, inv_a, p, q, r, sigma_n, k}): b200vton_cfg_solver_step_rows' result;
+ *   3 DDPM (row {gs, sb, inv_sa, c0, c1, sigma, phi, 0}): b200vton_cfg_ddpm_step_rows' result, or under CFG with
+ *     phi > 0 b200vton_cfg_rescale_ddpm_step's result on that sample alone.
+ * noise (may be null) enters DDPM and DDIM rows only; x0_prev (required) is read and rewritten by DPM-Solver++ rows only.
+ * Kind values are not checked on the device. coef_stride 0 or >= 8; fp16 pointers 2-byte aligned, coef and kinds 4. */
+int b200vton_cfg_step_mixed_rows(const void* eps, int ldc, int B, int C, int H, int W, const void* latents,
+                                 const void* noise, void* x0_prev, const void* coef, int coef_stride, const void* kinds,
+                                 int do_cfg, void* out, void* stream);
+
 /* Pre-processing of the inpainting inputs in one launch (diffusers VaeImageProcessor.preprocess for image and mask,
  * the masked image and the latent-resolution mask: src/tryon_pipeline.py:1588-1602, 940-943). image: [B,3,H,W] fp32;
  * mask: [B,mask_channels,H,W] fp32 (1, or 3 = RGB converted to grayscale); image_min: device scalar = min(image)
