@@ -8,12 +8,17 @@
 // A CTA computes 128 x BN output tiles, one after another: the grid is min(tiles, SMs) and CTA b takes tiles b,
 // b + gridDim.x, ... (n fastest, so neighbouring CTAs share an A slab in L2). Warps 0..7 are two consumer warpgroups
 // (rows 0..63 / 64..127 of the tile) that issue m64nBNk16 (k8 for TF32) wgmma from 128B-swizzled shared memory into
-// register accumulators; warp 8 (in a warpgroup of its own, which gives its registers to the consumers) is the TMA
-// producer. The conv walks K as 9 taps x Cin/64 slabs with a 4-D tensor map over [B,H,W,C]; out-of-bounds box elements
-// are zero-filled by TMA, which is the conv's zero padding. After a tile's K loop each consumer thread runs the fused
-// epilogue on its own accumulator fragment (gemm_common.cuh) and stores 16 bytes at a time. The epilogue does not touch
-// shared memory, so the producer runs on into the next tile's slabs meanwhile and the operand ring is full again when
-// the consumers come back: only a CTA's first tile waits for a load.
+// register accumulators; warp 8 (in a warpgroup of its own, which gives most of its registers to the consumers) is the
+// TMA producer. The conv walks K as 9 taps x Cin/64 slabs with a 4-D tensor map over [B,H,W,C]; out-of-bounds box
+// elements are zero-filled by TMA, which is the conv's zero padding. The producer runs on into the next tile's slabs
+// while the consumers finish a tile, so only a CTA's first tile waits for a load.
+// The fp16 epilogue is split in two (gemm_common.cuh). After a tile's K loop each consumer thread does the register
+// half on its own accumulator fragment (bias, activation or GEGLU, time embedding, shortcut, residual) and writes the
+// tile to a shared-memory staging tile, then goes straight on to the next tile's K loop. Warps 9..11 of the producer's
+// warpgroup, which used to only give up their registers, do the memory half: they store the staged tile to global
+// memory 16 bytes at a time while the next K loop runs, and then bulk-copy the residual rows of the tile after it into
+// the staging tile, so it is there when that tile is staged. Two mbarriers hand the staging tile back and forth
+// (`staged`, `ready`). The fp32-output kinds keep their epilogue in the consumers and store from the fragment.
 // e4m3 linears (KIND_E4M3, the opt-in FP8 mode): a 128-byte slab row holds 128 e4m3 values, so the ring, the
 // descriptors and the 32-byte MMA step are those of the fp16 kind; the MMA is m64nNk32 e4m3 x e4m3 -> fp32 and the
 // epilogue scales each accumulator by its row's and column's scale before the fp16 epilogue below. The tensor core
@@ -31,20 +36,27 @@ namespace vton {
 
 enum : int { KIND_F16 = 0, KIND_F16IN_F32OUT = 1, KIND_TF32 = 2, KIND_E4M3 = 3 };
 
-template <int BN, int STAGES>
+constexpr bool f16_out(int kind) { return kind == KIND_F16 || kind == KIND_E4M3; }
+
+// Operand ring, then (fp16 output) the staging tile of the epilogue, the barriers and the store warps' row tables.
+template <int BN, int STAGES, bool GEGLU, int KIND>
 struct SmemLayout {
   static constexpr int B_BYTES = BN * 128;              // BN rows x 128 B (64 halves, 32 floats or 128 e4m3)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;   // the barriers follow the operand ring
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;     // barriers + alignment slack
+  static constexpr int STAGING_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int STAGING_BYTES = f16_out(KIND) ? StagingTile<BN, GEGLU>::BYTES : 0;
+  static constexpr int BAR_OFFSET = STAGING_OFFSET + STAGING_BYTES;   // full[STAGES], empty[STAGES], staged, ready
+  static constexpr int ROWS_OFFSET = BAR_OFFSET + 256;                // 2 x 128 int32 output rows
+  static constexpr int TOTAL = ROWS_OFFSET + (f16_out(KIND) ? 2 * BM * 4 : 0) + 1024;   // + alignment slack
 };
 
-// 2 consumer warpgroups + the producer's warpgroup (warp 8 loads; warps 9..11 only hand over their registers). ptxas
-// allots registers per whole warpgroup, 65536 / 384 = 168 a thread, which does not hold a 128-float accumulator and the
-// epilogue; so the producer's warpgroup drops to 40 and the consumers rise to 232 (128 * 40 + 256 * 232 <= 65536).
+// 2 consumer warpgroups + the producer's warpgroup (warp 8 loads; warps 9..11 store the fp16 epilogue, or only hand
+// over their registers for the fp32-output kinds). ptxas allots registers per whole warpgroup, 168 a thread at launch
+// (64512 for the CTA), which does not hold a 128-float accumulator and the epilogue; so the producer's warpgroup drops
+// to 56 and the consumers rise to 224 (128 * 56 + 256 * 224 = 64512).
 constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_PRODUCER_REGS = 40;
-constexpr int GEMM_CONSUMER_REGS = 232;
+constexpr int GEMM_PRODUCER_REGS = 56;
+constexpr int GEMM_CONSUMER_REGS = 224;
 
 template <int BN>
 constexpr int E4M3_SUB = BN == 256 ? 64 : (BN == 192 ? 96 : BN);
@@ -54,20 +66,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmS0, const __grid_constant__ CUtensorMap tmS1,
                  const __grid_constant__ CUtensorMap tmBs, const GemmParams p) {
-  using L = SmemLayout<BN, STAGES>;
+  using L = SmemLayout<BN, STAGES, GEGLU, KIND>;
   constexpr int KBK = KIND == KIND_TF32 ? 32 : (KIND == KIND_E4M3 ? 128 : 64);   // channels per 128-byte slab row
-  constexpr bool F16_EPI = KIND == KIND_F16 || KIND == KIND_E4M3;
+  constexpr bool F16_EPI = f16_out(KIND);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  // staging tile handshake for tile j of the CTA's schedule: `ready` completes phase j when the store warps have read
+  // tile j - 1 out of the staging tile and tile j's residual has landed in it, `staged` when both consumer warpgroups
+  // have written tile j
+  const uint32_t staged_bar = bar_base + 8u * (2 * STAGES);
+  const uint32_t ready_bar = bar_base + 8u * (2 * STAGES + 1);
+  const uint32_t staging = smem_base + L::STAGING_OFFSET;
+  // the staging tile and the store warps' row tables as pointers (from the 1024-aligned base)
+  auto staging_ptr = [&]() { return smem_raw + (smem_base - smem_u32(smem_raw)) + L::STAGING_OFFSET; };
+  auto row_table = [&]() { return reinterpret_cast<int*>(smem_raw + (smem_base - smem_u32(smem_raw)) + L::ROWS_OFFSET); };
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int total_slabs = p.slabs_main + (SC ? p.slabs_sc : 0);
 
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 8 * 32) {   // warp 8, lane 0
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (SC) {
@@ -78,6 +97,10 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+    }
+    if (F16_EPI) {
+      mbar_init(staged_bar, 256);   // every consumer thread, after its staging stores
+      mbar_init(ready_bar, EpilogueStore<BN, GEGLU>::THREADS);
     }
     fence_barrier_init();
   }
@@ -90,7 +113,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp >= 8) {
     // ===================== TMA producer =====================
     setmaxnreg_dec<GEMM_PRODUCER_REGS>();
-    if (warp == 8 && lane == 0) {
+    if (threadIdx.x == 8 * 32) {
+      const int total_slabs = p.slabs_main + (SC ? p.slabs_sc : 0);
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int n0 = (tile % p.n_tiles) * BN;
@@ -129,6 +153,9 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       }
+    } else if (F16_EPI && warp > 8) {
+      // ===================== store warps: the memory half of the fp16 epilogue =====================
+      EpilogueStore<BN, GEGLU>::run(p, staging, staging_ptr(), row_table(), staged_bar, ready_bar, threadIdx.x - 9 * 32);
     }
     return;
   }
@@ -136,6 +163,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // ===================== consumers: two warpgroups, 64 accumulator rows each =====================
   setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   const int wg = warp >> 2;
+  const int lane = threadIdx.x & 31;
   const int r_local = wg * 64 + ((warp & 3) << 4) + (lane >> 2);   // the thread's first fragment row (the other: + 8)
   float acc[BN / 2];
   float acc_sc[BN / 2];   // shortcut accumulator (dead when !SC)
@@ -200,20 +228,28 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   };
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    EpilogueF16<BN, GEGLU, SC, KIND == KIND_E4M3> epi;   // fp16 output: bias / residual loads fly during the K loop
+    EpilogueF16<BN, GEGLU, SC, KIND == KIND_E4M3> epi;   // fp16 output: the bias loads fly during the K loop
     if constexpr (F16_EPI) epi.begin(p, tile / p.n_tiles, tile % p.n_tiles, r_local);
     if constexpr (KIND == KIND_E4M3) {
       run_slabs_promoted(acc, 0, p.slabs_main);
     } else {
       run_slabs(acc, 0, p.slabs_main);
-      if constexpr (SC) run_slabs(acc_sc, p.slabs_main, total_slabs);
+      if constexpr (SC) run_slabs(acc_sc, p.slabs_main, p.slabs_main + p.slabs_sc);
       wgmma_wait<0>();
       fence_regs(acc);
       if (SC) fence_regs(acc_sc);
       release(it - 1);
     }
     if constexpr (F16_EPI) {
-      epi.finish(p, acc, acc_sc);
+      // The store warps stored tile j - 1 and copied this tile's residual into the staging tile while this tile's K loop
+      // ran; once both are done, stage this tile and go straight on to the next tile's slabs.
+      mbar_wait(ready_bar, ((tile - blockIdx.x) / gridDim.x) & 1);   // phase j for tile j of this CTA's schedule
+      if (!GEGLU && p.act_gelu) epi.template stage<true, true>(p, acc, acc_sc, r_local, staging);
+      else if (!GEGLU && p.rowvec) epi.template stage<false, true>(p, acc, acc_sc, r_local, staging);
+      else epi.template stage<false, false>(p, acc, acc_sc, r_local, staging);
+      mbar_arrive(staged_bar);
+      if (tile + static_cast<int>(gridDim.x) >= p.total_tiles)   // the CTA's last tile: help the store warps store it
+        EpilogueStore<BN, GEGLU>::help_store_last(p, tile, staging_ptr(), row_table(), staged_bar, threadIdx.x);
     } else {
       epilogue_f32<BN>(p, tile / p.n_tiles, tile % p.n_tiles, r_local, acc);
     }
@@ -226,7 +262,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 template <int BN, int STAGES, bool GEGLU, bool SC, int KIND>
 static int launch_variant(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmS0,
                           const CUtensorMap& tmS1, const CUtensorMap& tmBs, const GemmParams& p, cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES>;
+  using L = SmemLayout<BN, STAGES, GEGLU, KIND>;
   static_assert(L::TOTAL <= 227 * 1024, "shared memory budget");
   auto kern = gemm_conv_kernel<BN, STAGES, GEGLU, SC, KIND>;
   static bool configured = false;
@@ -305,7 +341,7 @@ static int dispatch(int bn, bool geglu, const CUtensorMap& tmA, const CUtensorMa
     case 128: return launch_variant<128, 6, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
     case 160: return launch_variant<160, 5, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
     case 192: return launch_variant<192, 4, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
-    case 256: return launch_variant<256, 4, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);
+    case 256: return launch_variant<256, 3, false, false, KIND>(tmA, tmB, tmS0, tmS1, tmBs, p, stream);   // + 64 KB staging
   }
   set_last_error("unsupported BN %d", bn);
   return kErrUnsupported;

@@ -106,52 +106,65 @@ __device__ __forceinline__ float2 ldg_h2(const __half* src) {
   return unpack_h2(__ldg(reinterpret_cast<const uint32_t*>(src)));
 }
 
-// Fused fp16 epilogue of one 128 x BN tile, straight from the wgmma accumulator fragment. The thread holds rows r_local
-// and r_local + 8 of the tile and, of every 8-column group i, columns 8i + 2q + {0,1} in acc[4i .. 4i+3] (q = lane & 3);
-// acc_sc (the shortcut accumulator) has the same layout, and the GEGLU gate of column c is column c + BN/2 of the same
-// thread. Per element, with the reference's fp16 rounding points:
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+// Bulk copy (no tensor map) of `bytes` (a multiple of 16, both addresses 16-byte aligned) from global to shared memory,
+// completing as transaction bytes on the mbarrier `bar`.
+__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar) : "memory");
+}
+
+// The fp16 tile between the two halves of the epilogue: 128 rows x OUT_COLS halves in shared memory, row-major in
+// 16-byte chunks, so that a residual row lands in it with one bulk copy. The consumers read and write it a quad at a
+// time (4 consecutive chunks of rows r and r + 1 in one 8-lane phase: conflict-free with 20 chunks per row, two-way
+// where a row holds a multiple of 8 chunks) and the store warps read 8 consecutive chunks of a row at a time.
+template <int BN, bool GEGLU>
+struct StagingTile {
+  static constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
+  static constexpr int CHUNKS_PER_ROW = OUT_COLS / 8;
+  static constexpr int BYTES = BM * OUT_COLS * 2;
+  __device__ static __forceinline__ uint32_t offset(int r, int chunk) {
+    return static_cast<uint32_t>(r * CHUNKS_PER_ROW + chunk) * 16u;
+  }
+};
+
+// Register half of the fp16 epilogue of one 128 x BN tile, straight from the wgmma accumulator fragment. The thread
+// holds rows r_local and r_local + 8 of the tile and, of every 8-column group i, columns 8i + 2q + {0,1} in
+// acc[4i .. 4i+3] (q = lane & 3); acc_sc (the shortcut accumulator) has the same layout, and the GEGLU gate of column c
+// is column c + BN/2 of the same thread. Per element, with the reference's fp16 rounding points:
 //   v = fp16(acc + bias); v = act(v); v = fp16(v + temb[sample]); v = fp16(fp16(acc_sc + bias_sc) + v); v = fp16(v + res)
 //   GEGLU: v = fp16(h) * fp16(gelu(fp16(g)))
 // Bias and time embedding are read in the fragment shape (one half2 per column pair, the bias once for both rows). The
-// packed half2 words of four 8-groups are then transposed across the quad, so each lane owns 8 contiguous columns of
-// one row: the residual is added and the result stored 16 bytes per lane, a quad filling 64 contiguous bytes of a row.
-// Column groups at or past N and rows outside the output are neither read nor stored.
+// packed half2 words of four 8-groups are then transposed across the quad, so each lane owns 8 contiguous columns of one
+// row; the residual of those 8 columns, which the store warps have copied into the staging tile during the K loop, is
+// added in place and the result written back, 16 bytes per lane.
 //
-// Only eight consumer warps share an SM, so a global load whose value is needed at once costs its whole latency, and a
-// load cannot be moved above an earlier store to `out` by the compiler (the two may alias). begin() therefore runs
-// before the tile's K loop: it maps the rows and issues the loads of the tile's bias words and of the first RES_AHEAD
-// chunks of the residual, which land while the tensor cores work. finish() runs after the K loop and keeps the residual
-// RES_AHEAD chunks ahead of the chunk it stores; a consumed chunk frees 16 accumulator registers for the 8 it loads.
+// Only eight consumer warps share an SM, so a global load whose value is needed at once costs its whole latency.
+// begin() therefore runs before the tile's K loop: it maps the rows and issues the loads of the tile's bias words,
+// which land while the tensor cores work.
 // SCALED (e4m3 operands): every accumulator is first scaled to (acc * a_scale[row]) * w_scale[col] in fp32; the row
 // scales are loaded in begin(), the column scales of an 8-group where it is scaled (L1 hits after the first row; BN/4
 // more registers held across the K loop would not fit at BN = 256). Everything after that is the fp16 epilogue unchanged.
 template <int BN, bool GEGLU, bool SC, bool SCALED = false>
 struct EpilogueF16 {
-  static constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
+  using Staging = StagingTile<BN, GEGLU>;
+  static constexpr int OUT_COLS = Staging::OUT_COLS;
   static constexpr int CHUNKS = OUT_COLS / 32;
   static constexpr bool HAS_RES = !GEGLU && !SC;   // a residual comes with neither GEGLU nor a fused shortcut
-  // SCALED: the e4m3 main loop holds a partial-sum accumulator beside acc, so the residual is loaded one chunk ahead only
-  static constexpr int RES_AHEAD = (!HAS_RES || SCALED) ? 1 : (CHUNKS < 4 ? CHUNKS : 4);
 
   int q, n0, out_n0, out_N;
   long long out_row[2];
   int sample[2];
   uint32_t bias[BN / 8];              // half2 of columns n0 + 8i + 2q + {0,1} (GEGLU: value and gate halves alike)
   uint32_t bias_sc[SC ? BN / 8 : 1];
-  uint4 res[2][RES_AHEAD];            // residual of chunk c in slot c % RES_AHEAD, in the transposed (stored) shape
   float a_scale[SCALED ? 2 : 1];      // row scales of rows r_local and r_local + 8
-
-  __device__ __forceinline__ int own_col(int c) const { return out_n0 + (4 * c + q) * 8; }   // this lane's 8-group of chunk c
-
-  __device__ __forceinline__ void load_res(const GemmParams& p, int c) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint4 u = make_uint4(0u, 0u, 0u, 0u);
-      if (p.residual && out_row[h] >= 0 && own_col(c) < out_N)
-        u = *reinterpret_cast<const uint4*>(p.residual + out_row[h] * p.ld_res + own_col(c));
-      res[h][c % RES_AHEAD] = u;
-    }
-  }
 
   __device__ __forceinline__ void begin(const GemmParams& p, int m_tile, int n_tile, int r_local) {
     q = threadIdx.x & 3;
@@ -170,19 +183,24 @@ struct EpilogueF16 {
       bias[i] = (p.bias && ok) ? __ldg(reinterpret_cast<const uint32_t*>(p.bias + n0 + i * 8 + 2 * q)) : 0u;
       if (SC) bias_sc[i] = (p.bias_sc && ok) ? __ldg(reinterpret_cast<const uint32_t*>(p.bias_sc + n0 + i * 8 + 2 * q)) : 0u;
     }
-    if (HAS_RES) {
-#pragma unroll
-      for (int c = 0; c < RES_AHEAD; ++c) load_res(p, c);
-    }
   }
 
-  __device__ __forceinline__ void finish(const GemmParams& p, const float (&acc)[BN / 2], const float (&acc_sc)[BN / 2]) {
+  // Writes the tile's fp16 output to the staging tile at shared address `staging`, which holds the tile's residual.
+  // ACT / ROWVEC: whether the activation / time-embedding code is compiled in at all. The caller picks the variant once
+  // per tile (act_gelu != 0 needs ACT, a rowvec needs ROWVEC), so the common path is straight-line code of a few
+  // instructions per column pair instead of a walk over rare branches inlined for every pair, which made the epilogue
+  // instruction-fetch bound.
+  template <bool ACT, bool ROWVEC>
+  __device__ __forceinline__ void stage(const GemmParams& p, const float (&acc)[BN / 2], const float (&acc_sc)[BN / 2],
+                                        int r_local, uint32_t staging) {
     // Rows outside the output (a conv box whose batch extent exceeds B, the ragged last M tile) carry a sample index past
     // the [B, ld_rowvec] time-embedding tensor: their values are never stored, so they must not read it either.
     const __half* rowvec_row[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
-      rowvec_row[h] = (p.rowvec && out_row[h] >= 0) ? p.rowvec + static_cast<long long>(sample[h]) * p.ld_rowvec : nullptr;
+      rowvec_row[h] = (ROWVEC && p.rowvec && out_row[h] >= 0)
+                          ? p.rowvec + static_cast<long long>(sample[h]) * p.ld_rowvec
+                          : nullptr;
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c) {
       if (out_n0 + c * 32 >= out_N) break;
@@ -222,13 +240,13 @@ struct EpilogueF16 {
               const float2 b = unpack_h2(bias[i]);
               v0 += b.x, v1 += b.y;
             }
-            if (p.act_gelu) {   // rare (Resampler FeedForward, CLIP MLPs)
+            if (ACT && p.act_gelu) {   // rare (Resampler FeedForward, CLIP MLPs)
               const float x0 = round_h(v0), x1 = round_h(v1);
               // 1: erf-GELU; 2: quick-GELU x * sigmoid(1.702 x) (the CLIP ViT-L text encoder's activation)
               v0 = p.act_gelu == 2 ? __fdividef(x0, 1.0f + __expf(-1.702f * x0)) : gelu_erf_fast(x0);
               v1 = p.act_gelu == 2 ? __fdividef(x1, 1.0f + __expf(-1.702f * x1)) : gelu_erf_fast(x1);
             }
-            if (rowvec_row[h] != nullptr && col_ok) {
+            if (ROWVEC && rowvec_row[h] != nullptr && col_ok) {
               const float2 t = ldg_h2(rowvec_row[h] + n0 + i * 8 + 2 * q);
               v0 = round_h(v0) + t.x, v1 = round_h(v1) + t.y;
             }
@@ -244,9 +262,9 @@ struct EpilogueF16 {
           w[g] = pack_h2(v0, v1);
         }
         quad_transpose(w, q);
-        if (out_row[h] < 0 || own_col(c) >= out_N) continue;
-        if (HAS_RES && p.residual) {
-          const uint4 u = res[h][c % RES_AHEAD];
+        const uint32_t slot = staging + Staging::offset(r_local + 8 * h, 4 * c + q);
+        if (HAS_RES && p.residual) {   // rows and columns outside the output hold stale words here: never stored
+          const uint4 u = ld_shared_v4(slot);
           const uint32_t r[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
           for (int j = 0; j < 4; ++j) {   // w already holds fp16(v)
@@ -254,9 +272,83 @@ struct EpilogueF16 {
             w[j] = pack_h2(a.x + d.x, a.y + d.y);
           }
         }
-        *reinterpret_cast<uint4*>(p.out + out_row[h] * p.ld_out + own_col(c)) = make_uint4(w[0], w[1], w[2], w[3]);
+        st_shared_v4(slot, w[0], w[1], w[2], w[3]);
       }
-      if (HAS_RES && c + RES_AHEAD < CHUNKS) load_res(p, c + RES_AHEAD);
+    }
+  }
+};
+
+// Memory half of the fp16 epilogue, on the 96 threads of warps 9..11 (e = 0..95), which walk the consumers' tile
+// schedule. For tile j they map its rows into a shared row table (double-buffered, so one named barrier per tile orders
+// its writes and reads). Once all of them are done reading tile j - 1 out of the staging tile, they bulk-copy tile j's
+// residual rows into it and arrive on `ready`, which completes when the copies have landed: the residual travels while
+// tile j's K loop runs and costs no registers, and the consumers add it as they stage the tile. When the consumers
+// have staged it (`staged`), the store warps store it 16 bytes at a time, 8 threads covering 128 contiguous bytes of a
+// row. A CTA's last tile has no K loop after it to hide its store behind, so the consumers join in and it is stored by
+// all 352 threads. Column groups at or past N and rows outside the output (a conv box whose batch extent exceeds B, the
+// ragged last M tile) are neither copied nor stored.
+template <int BN, bool GEGLU>
+struct EpilogueStore {
+  using Staging = StagingTile<BN, GEGLU>;
+  static constexpr int THREADS = 96;
+  static constexpr int CPR = Staging::CHUNKS_PER_ROW;
+  static constexpr int UNITS = BM * CPR;   // 16-byte chunks per tile
+
+  // Thread t of n stores chunks t, t + n, ... of the staged tile; rows: the tile's output rows (-1 = outside).
+  __device__ static __forceinline__ void store(const GemmParams& p, const uint8_t* staging_ptr, const int* rows, int out_n0,
+                                               int out_N, int t, int n) {
+#pragma unroll 4
+    for (int u = t; u < UNITS; u += n) {
+      const int r = u / CPR, chunk = u % CPR;
+      const int row = rows[r];
+      const int col = out_n0 + chunk * 8;
+      if (row >= 0 && col < out_N)
+        *reinterpret_cast<uint4*>(p.out + static_cast<long long>(row) * p.ld_out + col) =
+            *reinterpret_cast<const uint4*>(staging_ptr + Staging::offset(r, chunk));
+    }
+  }
+
+  // The consumers' share (thread t of 256) of storing `tile`, the CTA's last, once both warpgroups have staged it.
+  __device__ static __forceinline__ void help_store_last(const GemmParams& p, int tile, const uint8_t* staging_ptr,
+                                                         const int* row_table, uint32_t staged_bar, int t) {
+    const int j = (tile - blockIdx.x) / gridDim.x;
+    mbar_wait(staged_bar, j & 1);
+    store(p, staging_ptr, row_table + (j & 1) * BM, (tile % p.n_tiles) * Staging::OUT_COLS, GEGLU ? p.N / 2 : p.N,
+          THREADS + t, THREADS + 256);
+  }
+
+  __device__ static __forceinline__ void run(const GemmParams& p, uint32_t staging, const uint8_t* staging_ptr,
+                                             int* row_table, uint32_t staged_bar, uint32_t ready_bar, int e) {
+    const int out_N = GEGLU ? p.N / 2 : p.N;
+    int j = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++j) {
+      const int m_tile = tile / p.n_tiles;
+      const int out_n0 = (tile % p.n_tiles) * Staging::OUT_COLS;
+      int* rows = row_table + (j & 1) * BM;
+      for (int r = e; r < BM; r += THREADS) {
+        long long out_row;
+        int sample;
+        map_row(p, m_tile, r, &out_row, &sample);
+        rows[r] = static_cast<int>(out_row);
+      }
+      named_bar_sync(1, THREADS);   // the row table is complete and nobody reads the staging tile any more
+      if (p.residual) {
+        fence_proxy_async_smem();   // the staging tile's generic reads before the copies' writes
+        const uint32_t row_bytes = (out_N - out_n0 < Staging::OUT_COLS ? out_N - out_n0 : Staging::OUT_COLS) * 2u;
+        uint32_t bytes = 0;
+        for (int r = e; r < BM; r += THREADS) bytes += rows[r] >= 0 ? row_bytes : 0u;
+        mbar_expect_tx(ready_bar, bytes);   // arrives, and expects this thread's copies
+        for (int r = e; r < BM; r += THREADS) {
+          if (rows[r] >= 0)
+            bulk_copy_g2s(staging + Staging::offset(r, 0), p.residual + static_cast<long long>(rows[r]) * p.ld_res + out_n0,
+                          row_bytes, ready_bar);
+        }
+      } else {
+        mbar_arrive(ready_bar);
+      }
+      mbar_wait(staged_bar, j & 1);
+      const bool last = tile + static_cast<int>(gridDim.x) >= p.total_tiles;
+      store(p, staging_ptr, rows, out_n0, out_N, e, last ? THREADS + 256 : THREADS);
     }
   }
 };
