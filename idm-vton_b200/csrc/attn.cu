@@ -32,6 +32,10 @@
 // Samples with a real segment 1 (b >= kv1_off, the longest CTAs) are scheduled before the zero-K/V samples.
 // With IP (the decoupled text + IP-token cross-attention), segment 1 has its own softmax and the CTA stores
 // fp16(fp16(O_0) + fp16(out_scale * fp16(O_1))).
+#include <cuda_fp8.h>
+
+#include <algorithm>
+
 #include "common.cuh"
 #include "host.h"
 #include "wgmma.cuh"
@@ -59,15 +63,22 @@ constexpr int FA_THREADS = 384;       // consumer warpgroups 0 and 1, producer w
 constexpr int FA_PRODUCER_REGS = 40;  // 128 * 40 + 256 * 232 = 64512 <= 65536 registers per SM
 constexpr int FA_CONSUMER_REGS = 232;
 constexpr uint32_t FA_BAR_TURN = 1;   // named barriers FA_BAR_TURN + wg: consumer wg may issue its MMAs (0 = __syncthreads)
+constexpr uint32_t FA_BAR_CVT = 3;    // KV8: the converting warps 9-11 have written a stage's fp16 K/V
+constexpr int FA_CVT_THREADS = 96;
 
-template <int R>
+// KV8: per stage, a staging area for a segment-1 tile in the FP8 garment K/V format (e4m3 K and V, 64 B x 128 rows
+// each, then the 128 K and 128 V exponents), and one more mbarrier per stage (stg_full)
+template <int R, bool KV8 = false>
 struct FlashSmem {
   static constexpr int STAGES = R == 1 ? 3 : 2;
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_K = OFF_Q + R * FA_REGION;
   static constexpr int OFF_V = OFF_K + STAGES * R * FA_REGION;
-  static constexpr int OFF_BAR = OFF_V + STAGES * R * FA_REGION;
-  static constexpr int TOTAL = OFF_BAR + 64 + 1024;
+  static constexpr int STG_Q = 128 * 64;                       // one e4m3 tile
+  static constexpr int STG_BYTES = KV8 ? 2 * STG_Q + 2 * 128 : 0;
+  static constexpr int OFF_STG = OFF_V + STAGES * R * FA_REGION;
+  static constexpr int OFF_BAR = OFF_STG + STAGES * STG_BYTES;
+  static constexpr int TOTAL = OFF_BAR + (KV8 ? 128 : 64) + 1024;
 };
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -76,16 +87,35 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
+// The FP8 garment K/V format (INTEGRATION.md, "FP8 garment K/V"): x = fp16(float(q) * 2^e) with q e4m3 and e one int8
+// per (token, 64-column group). fp16(2^e) for e in [-24, 8] (subnormal below -14).
+__device__ __forceinline__ uint32_t kv8_scale_h2(int e) {
+  const uint32_t hb = e >= -14 ? static_cast<uint32_t>(e + 15) << 10 : 1u << (e + 24);
+  return hb | (hb << 16);
+}
+// Two e4m3 codes (low byte first) -> fp16x2, times fp16(2^e) in one rounding: the rule's bits, since both factors are
+// exact fp16 numbers
+__device__ __forceinline__ uint32_t kv8_dequant2(uint32_t codes, uint32_t scale_h2) {
+  const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(codes & 0xffffu), __NV_E4M3);
+  __half2 v(r);
+  const __half2 s = *reinterpret_cast<const __half2*>(&scale_h2);
+  v = __hmul2_rn(v, s);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
 // KS: Q K^T k-steps (D / 16); IP: segment 1 has a softmax of its own (the text + IP-token cross-attention, D = 64);
 // R: 64-column regions per head; DN: P V tile width (64 for D <= 64, 96 otherwise). D > 64 (the CLIP image tower)
 // and IP do not overlap a warpgroup's softmax with its own P V: S, P and a 96-wide O (or O and the kept fp16 O_0) do not
 // fit the registers together.
-template <int KS, bool IP = false, int R = (KS + 3) / 4, int DN = (KS <= 4 ? 64 : 96)>
-__global__ void __launch_bounds__(FA_THREADS, 1)
-flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-             const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-             const __grid_constant__ CUtensorMap tmV1, const FlashParams p) {
-  using SM = FlashSmem<R>;
+// KV8 (D = 64 without IP only): segment 1 is in the FP8 garment K/V format. The TMA thread loads a segment-1 tile's e4m3
+// K / V and exponents into the stage's staging area (stg_full), and the producer warpgroup's warps 9-11 write it as
+// fp16 into the stage's 128B-swizzled K / V slots, then arrive on kv_full: the consumers read what they read for fp16.
+template <int KS, bool IP, int R, int DN, bool KV8>
+__device__ __forceinline__ void flash_body(const CUtensorMap* tmQ, const CUtensorMap* tmK0, const CUtensorMap* tmV0,
+                                           const CUtensorMap* tmK1, const CUtensorMap* tmV1, const CUtensorMap* tmE,
+                                           const FlashParams p) {
+  static_assert(!KV8 || (KS == 4 && !IP && R == 1 && DN == 64), "the FP8 segment 1 is for D = 64 without IP");
+  using SM = FlashSmem<R, KV8>;
   constexpr int ST = SM::STAGES;
   constexpr bool OVERLAP = DN == 64 && !IP;   // IP runs two tiles, one per softmax: nothing to overlap
   extern __shared__ uint8_t smem_raw[];
@@ -94,6 +124,7 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   const uint32_t q_full = bar_base;
   auto kv_full = [&](int s) { return bar_base + 8u * (1 + s); };
   auto kv_empty = [&](int s) { return bar_base + 8u * (1 + ST + s); };
+  auto stg_full = [&](int s) { return bar_base + 8u * (1 + 2 * ST + s); };   // KV8 only
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -112,16 +143,18 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
     for (int s = 0; s < ST; ++s) {
       mbar_init(kv_full(s), 1);
       mbar_init(kv_empty(s), 2);   // one arrival per consumer warpgroup
+      if constexpr (KV8) mbar_init(stg_full(s), 1);
     }
     fence_barrier_init();
   }
   if (threadIdx.x == 256) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK0);
-    tma_prefetch_desc(&tmV0);
+    tma_prefetch_desc(tmQ);
+    tma_prefetch_desc(tmK0);
+    tma_prefetch_desc(tmV0);
     if (p.N1 > 0) {
-      tma_prefetch_desc(&tmK1);
-      tma_prefetch_desc(&tmV1);
+      tma_prefetch_desc(tmK1);
+      tma_prefetch_desc(tmV1);
+      if constexpr (KV8) tma_prefetch_desc(tmE);
     }
   }
   // Programmatic dependent launch: Q/K/V (and kv1_base / kv1_rows) are written by the previous kernels of the stream
@@ -152,11 +185,23 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
       mbar_expect_tx(q_full, R * FA_REGION);
 #pragma unroll
       for (int r = 0; r < R; ++r)
-        tma_load_3d(smem_base + SM::OFF_Q + r * FA_REGION, &tmQ, q_full, h * p.D + r * 64, q_tile * 128, b);
+        tma_load_3d(smem_base + SM::OFF_Q + r * FA_REGION, tmQ, q_full, h * p.D + r * 64, q_tile * 128, b);
       // K/V tile j into stage j % ST, once both consumers have released the stage's previous tile
       for (int j = 0; j < total; ++j) {
         const int stage = j % ST;
         if (j >= ST) mbar_wait(kv_empty(stage), ((j / ST) - 1) & 1);
+        if constexpr (KV8) {
+          if (j >= tiles0) {   // e4m3 K, V and their exponents (K group h, V group H + h) into the staging area
+            const uint32_t stg = smem_base + SM::OFF_STG + stage * SM::STG_BYTES;
+            const int key0 = (j - tiles0) * 128;
+            mbar_expect_tx(stg_full(stage), SM::STG_BYTES);
+            tma_load_3d(stg, tmK1, stg_full(stage), h * 64, key0, idx1);
+            tma_load_3d(stg + SM::STG_Q, tmV1, stg_full(stage), h * 64, key0, idx1);
+            tma_load_3d(stg + 2 * SM::STG_Q, tmE, stg_full(stage), key0, h, idx1);
+            tma_load_3d(stg + 2 * SM::STG_Q + 128, tmE, stg_full(stage), key0, p.H + h, idx1);
+            continue;
+          }
+        }
         mbar_expect_tx(kv_full(stage), 2 * R * FA_REGION);
 #pragma unroll
         for (int r = 0; r < R; ++r) {
@@ -164,12 +209,40 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
           const uint32_t vdst = smem_base + SM::OFF_V + (stage * R + r) * FA_REGION;
           const int col = h * p.D + r * 64;
           if (j < tiles0) {
-            tma_load_3d(kdst, &tmK0, kv_full(stage), col, j * 128, b);
-            tma_load_3d(vdst, &tmV0, kv_full(stage), col, j * 128, b);
+            tma_load_3d(kdst, tmK0, kv_full(stage), col, j * 128, b);
+            tma_load_3d(vdst, tmV0, kv_full(stage), col, j * 128, b);
           } else {
-            tma_load_3d(kdst, &tmK1, kv_full(stage), col, (j - tiles0) * 128, idx1);
-            tma_load_3d(vdst, &tmV1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+            tma_load_3d(kdst, tmK1, kv_full(stage), col, (j - tiles0) * 128, idx1);
+            tma_load_3d(vdst, tmV1, kv_full(stage), col, (j - tiles0) * 128, idx1);
           }
+        }
+      }
+    } else if constexpr (KV8) {
+      if (warp >= 9) {
+        // Warps 9-11 turn each staged segment-1 tile into fp16: 2 x 128 rows x 8 chunks of 16 B, chunk c of row r at
+        // byte r * 128 + ((c ^ (r & 7)) << 4) of the slot (what a SWIZZLE_128B TMA load writes). The staging area of
+        // stage s is refilled only after both consumers released the slot (kv_empty), which is after this arrival.
+        const int t = threadIdx.x - 288;
+        for (int j = tiles0; j < total; ++j) {
+          const int stage = j % ST;
+          mbar_wait(stg_full(stage), ((j - tiles0) / ST) & 1);
+          const uint32_t stg = smem_base + SM::OFF_STG + stage * SM::STG_BYTES;
+#pragma unroll 1   // 40 registers after setmaxnreg.dec: an unrolled loop spills
+          for (int c = t; c < 2 * 128 * 8; c += FA_CVT_THREADS) {
+            const int kv = c >> 10, r = (c >> 3) & 127, ch = c & 7;
+            uint32_t lo, hi;
+            int e;
+            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(lo), "=r"(hi) : "r"(stg + kv * SM::STG_Q + r * 64 + ch * 8));
+            asm volatile("ld.shared.s8 %0, [%1];" : "=r"(e) : "r"(stg + 2 * SM::STG_Q + kv * 128 + r));
+            const uint32_t sc = kv8_scale_h2(e);
+            const uint32_t dst = smem_base + (kv ? SM::OFF_V : SM::OFF_K) + stage * FA_REGION + r * 128 + ((ch ^ (r & 7)) << 4);
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(kv8_dequant2(lo, sc)),
+                         "r"(kv8_dequant2(lo >> 16, sc)), "r"(kv8_dequant2(hi, sc)), "r"(kv8_dequant2(hi >> 16, sc))
+                         : "memory");
+          }
+          fence_proxy_async_smem();   // generic-proxy writes, read by wgmma through the async proxy
+          named_bar_sync(FA_BAR_CVT, FA_CVT_THREADS);
+          if (t == 0) mbar_arrive(kv_full(stage));
         }
       }
     }
@@ -452,6 +525,23 @@ flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
   }
 }
 
+template <int KS, bool IP = false, int R = (KS + 3) / 4, int DN = (KS <= 4 ? 64 : 96)>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
+             const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
+             const __grid_constant__ CUtensorMap tmV1, const FlashParams p) {
+  flash_body<KS, IP, R, DN, false>(&tmQ, &tmK0, &tmV0, &tmK1, &tmV1, nullptr, p);
+}
+
+// Self + garment attention of the try-on blocks with the garment K/V (segment 1) in the FP8 format: tmK1 / tmV1 are
+// one-byte maps of the e4m3 K / V (box 64 x 128, no swizzle), tmE the exponents [B1, 2H, lde] (box 128 x 1 x 1).
+__global__ void __launch_bounds__(FA_THREADS, 1)
+flash_kv8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
+                 const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
+                 const __grid_constant__ CUtensorMap tmV1, const __grid_constant__ CUtensorMap tmE, const FlashParams p) {
+  flash_body<4, false, 1, 64, true>(&tmQ, &tmK0, &tmV0, &tmK1, &tmV1, &tmE, p);
+}
+
 // Tuning switches of other attention kernels of this library's C ABI. There is one attention kernel here, which always
 // runs the ping-pong schedule with 128-query tiles and ex2.approx, so the options "attention_pingpong",
 // "attention_q_tiles" and "attention_poly_exp" are accepted and have no effect.
@@ -591,6 +681,151 @@ int cross_attn_impl(const void* q, long long ldq, const void* kt, const void* vt
   p.out_scale = Ni > 0 ? ip_scale : 1.f;
   return flash(q, ldq, kt, vt, ldkv_t, Ni > 0 ? ki : nullptr, Ni > 0 ? vi : nullptr, ldkv_i, B, out, ldo, p, stream,
                Ni > 0);
+}
+
+// Self + garment attention with the garment K/V (segment 1) in the FP8 format: k1 / v1 e4m3 [B1, N1, >= H*64] (row
+// stride ldkv1 bytes), e1 int8 exponents [B1, 2H, lde1] (group h = K head h, group H + h = V head h). Segment 1 as in
+// attn_impl (kv1_mod / kv1_base) or, with kv1_rows, as in attn_rows_impl.
+int attn_kv8_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+                  const void* v1, long long ldkv1, const void* e1, long long lde1, void* out, long long ldo, int B, int H,
+                  int Nq, int N0, int N1, int B1, int kv1_off, int kv1_mod, const void* kv1_base, const void* kv1_rows,
+                  float scale, int accumulate, cudaStream_t stream) {
+  VTON_CHECK_ARG(B > 0 && H > 0 && Nq > 0 && N0 > 0 && N1 > 0 && B1 > 0,
+                 "attention_kv8: bad sizes B=%d H=%d Nq=%d N0=%d N1=%d B1=%d", B, H, Nq, N0, N1, B1);
+  VTON_CHECK_ARG(q && k0 && v0 && k1 && v1 && e1 && out, "attention_kv8: null pointer");
+  VTON_CHECK_ARG(ldq % 8 == 0 && ldkv0 % 8 == 0 && ldo % 8 == 0, "attention_kv8: fp16 row strides must be multiples of 8");
+  VTON_CHECK_ARG(ldkv1 % 16 == 0 && ldkv1 >= 64LL * H, "attention_kv8: ldkv1 %lld must be a multiple of 16 and >= 64*H",
+                 ldkv1);
+  VTON_CHECK_ARG(lde1 % 16 == 0 && lde1 >= N1, "attention_kv8: lde1 %lld must be a multiple of 16 and >= N1 = %d", lde1,
+                 N1);
+  VTON_CHECK_ARG(aligned_to(out, 4), "attention_kv8: out must be 4-byte aligned (stored two halves at a time)");
+  VTON_CHECK_ARG(aligned_to(kv1_rows, 4), "attention_kv8: kv1_rows must be 4-byte aligned (int32)");
+  VTON_CHECK_ARG(kv1_off >= 0 && kv1_off < B, "attention_kv8: kv1_off %d outside [0, B=%d)", kv1_off, B);
+  VTON_CHECK_ARG(B <= 65535 && H <= 65535, "attention_kv8: grid too large");
+  FlashParams p{};
+  p.B = B;
+  p.H = H;
+  p.Nq = Nq;
+  p.N0 = N0;
+  p.N1 = N1;
+  p.D = 64;
+  p.kv1_off = kv1_off;
+  p.kv1_count = kv1_rows || kv1_mod <= 0 ? B1 : kv1_mod;
+  p.kv1_base = kv1_rows ? nullptr : static_cast<const int*>(kv1_base);
+  p.kv1_rows = static_cast<const int*>(kv1_rows);
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.accumulate = accumulate;
+  p.out_scale = 1.f;
+  p.out = static_cast<__half*>(out);
+  p.ld_out = static_cast<int>(ldo);
+  CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1, tmE;
+  const int cols = H * 64;
+  if (int e = encode_tokens(&tmQ, q, ldq, cols, Nq, B)) return e;
+  if (int e = encode_tokens(&tmK0, k0, ldkv0, cols, N0, B)) return e;
+  if (int e = encode_tokens(&tmV0, v0, ldkv0, cols, N0, B)) return e;
+  {
+    const uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(N1), static_cast<uint64_t>(B1)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(ldkv1), static_cast<uint64_t>(ldkv1) * N1};
+    const uint32_t box[3] = {64, 128, 1};
+    if (int e = encode_tmap_u8(&tmK1, k1, 3, dims, strides, box, 0)) return e;
+    if (int e = encode_tmap_u8(&tmV1, v1, 3, dims, strides, box, 0)) return e;
+  }
+  {
+    const uint64_t dims[3] = {static_cast<uint64_t>(lde1), static_cast<uint64_t>(2 * H), static_cast<uint64_t>(B1)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(lde1), static_cast<uint64_t>(lde1) * 2 * H};
+    const uint32_t box[3] = {128, 1, 1};
+    if (int e = encode_tmap_u8(&tmE, e1, 3, dims, strides, box, 0)) return e;
+  }
+  using SM = FlashSmem<1, true>;
+  static bool configured = false;
+  if (!configured) {
+    VTON_CUDA(cudaFuncSetAttribute(flash_kv8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
+    configured = true;
+  }
+  dim3 grid((Nq + 127) / 128, H, B);
+  VTON_CUDA(launch_kernel(flash_kv8_kernel, grid, dim3(FA_THREADS), SM::TOTAL, stream, tmQ, tmK0, tmV0, tmK1, tmV1, tmE, p));
+  count_launch();
+  return kOk;
+}
+
+// The FP8 garment K/V quantizer. A warp takes 4 (token, group) items, 8 lanes each (8 values per lane); items run over
+// [rows, G, lde] with the token fastest, so the exponent stores of a warp are contiguous. Items with n >= Ng write the
+// exponent padding (0) only.
+__global__ void __launch_bounds__(256) quantize_kv_e4m3_kernel(const __half* __restrict__ x, long long ldx, int rows,
+                                                                int Ng, int G, int lde, uint8_t* __restrict__ q,
+                                                                long long ldq, int8_t* __restrict__ e_out) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int lane = threadIdx.x & 31, sub = lane & 7;
+  const long long n_items = static_cast<long long>(rows) * G * lde;
+  const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  for (long long base = (static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 4;
+       base < n_items; base += warps * 4) {
+    const long long it = base + (lane >> 3);
+    const bool valid = it < n_items;
+    const int n = valid ? static_cast<int>(it % lde) : 0;
+    const long long rg = valid ? it / lde : 0;   // row * G + g
+    const int g = static_cast<int>(rg % G);
+    const bool tok = valid && n < Ng;
+    const long long m = (rg / G) * Ng + n;
+    float v[8];
+    float amax = 0.f;
+    if (tok) {
+      const uint4 raw = *reinterpret_cast<const uint4*>(x + m * ldx + g * 64 + sub * 8);
+      const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float2 f = unpack_h2(w[i]);
+        v[2 * i] = f.x;
+        v[2 * i + 1] = f.y;
+        amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
+    // smallest e with amax <= 448 * 2^e: amax = 1.f * 2^E, 448 = 1.75 * 2^8
+    int e = 0;
+    if (amax > 0.f) {
+      const uint32_t bits = __float_as_uint(amax);
+      const int E = static_cast<int>((bits >> 23) & 0xff) - 127;
+      e = max(E - ((bits & 0x7fffffu) <= 0x600000u ? 8 : 7), -24);
+    }
+    if (tok) {
+      const float inv = __uint_as_float(static_cast<uint32_t>(127 - e) << 23);   // 2^-e, exact products
+      uint32_t packed[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const __nv_fp8x2_storage_t a =
+            __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(v[4 * i], inv), __fmul_rn(v[4 * i + 1], inv)), __NV_SATFINITE, __NV_E4M3);
+        const __nv_fp8x2_storage_t b =
+            __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(v[4 * i + 2], inv), __fmul_rn(v[4 * i + 3], inv)), __NV_SATFINITE, __NV_E4M3);
+        packed[i] = static_cast<uint32_t>(a) | (static_cast<uint32_t>(b) << 16);
+      }
+      *reinterpret_cast<uint2*>(q + m * ldq + g * 64 + sub * 8) = make_uint2(packed[0], packed[1]);
+    }
+    if (valid && sub == 0) e_out[rg * lde + n] = static_cast<int8_t>(tok ? e : 0);
+  }
+}
+
+int quantize_kv_e4m3_impl(const void* x, long long ldx, int M, int G, int Ng, void* q, long long ldq, void* e,
+                          long long lde, cudaStream_t stream) {
+  VTON_CHECK_ARG(M > 0 && G > 0 && Ng > 0 && M % Ng == 0, "quantize_kv_e4m3: bad sizes M=%d G=%d Ng=%d (M must be a "
+                 "multiple of Ng)", M, G, Ng);
+  VTON_CHECK_ARG(x && q && e, "quantize_kv_e4m3: null pointer");
+  VTON_CHECK_ARG(ldx % 8 == 0 && ldx >= 64LL * G && aligned_to(x, 16),
+                 "quantize_kv_e4m3: x must be 16-byte aligned with ldx a multiple of 8 and >= 64*G");
+  VTON_CHECK_ARG(ldq % 8 == 0 && ldq >= 64LL * G && aligned_to(q, 8),
+                 "quantize_kv_e4m3: q must be 8-byte aligned with ldq a multiple of 8 and >= 64*G");
+  VTON_CHECK_ARG(lde >= Ng && lde <= (1LL << 30), "quantize_kv_e4m3: lde %lld must be >= Ng = %d", lde, Ng);
+  const int rows = M / Ng;
+  const long long items = static_cast<long long>(rows) * G * lde;
+  const long long blocks = std::min<long long>((items + 31) / 32, 32LL * num_sms());
+  VTON_CUDA(launch_kernel(quantize_kv_e4m3_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream,
+                          static_cast<const __half*>(x), ldx, rows, Ng, G, static_cast<int>(lde),
+                          static_cast<uint8_t*>(q), ldq, static_cast<int8_t*>(e)));
+  count_launch();
+  return kOk;
 }
 
 // Encoder self-attention of the CLIP towers around the denoising loop: the ViT-H image encoder (16 heads of 80, 257

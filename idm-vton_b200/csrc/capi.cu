@@ -32,6 +32,12 @@ int attn_impl(const void* q, long long ldq, const void* k0, const void* v0, long
 int attn_rows_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
                    const void* v1, long long ldkv1, void* out, long long ldo, int B, int H, int Nq, int N0, int N1,
                    int B1, int kv1_off, const void* kv1_rows, float scale, int accumulate, cudaStream_t stream);
+int attn_kv8_impl(const void* q, long long ldq, const void* k0, const void* v0, long long ldkv0, const void* k1,
+                  const void* v1, long long ldkv1, const void* e1, long long lde1, void* out, long long ldo, int B, int H,
+                  int Nq, int N0, int N1, int B1, int kv1_off, int kv1_mod, const void* kv1_base, const void* kv1_rows,
+                  float scale, int accumulate, cudaStream_t stream);
+int quantize_kv_e4m3_impl(const void* x, long long ldx, int M, int G, int Ng, void* q, long long ldq, void* e,
+                          long long lde, cudaStream_t stream);
 int groupnorm_impl(const void* x0, int C0, const void* x1, int C1, int B, int HW, const void* gamma, const void* beta,
                    float eps, int silu, void* stats_ws, void* out, cudaStream_t stream);
 int layernorm_impl(const void* x, long long ldx, int rows, int C, const void* gamma, const void* beta, float eps,
@@ -146,6 +152,19 @@ int b200vton_attention_rows(const void* q, int64_t ldq, const void* k0, const vo
                             int B1, int kv1_off, const void* kv1_rows, float scale, int accumulate, void* stream) {
   return vton::attn_rows_impl(q, ldq, k0, v0, ldkv0, k1, v1, ldkv1, out, ldo, B, H, Nq, N0, N1, B1, kv1_off, kv1_rows,
                               scale, accumulate, S(stream));
+}
+
+int b200vton_attention_kv8(const void* q, int64_t ldq, const void* k0, const void* v0, int64_t ldkv0, const void* k1,
+                           const void* v1, int64_t ldkv1, const void* e1, int64_t lde1, void* out, int64_t ldo, int B,
+                           int H, int Nq, int N0, int N1, int B1, int kv1_off, int kv1_mod, const void* kv1_base,
+                           const void* kv1_rows, float scale, int accumulate, void* stream) {
+  return vton::attn_kv8_impl(q, ldq, k0, v0, ldkv0, k1, v1, ldkv1, e1, lde1, out, ldo, B, H, Nq, N0, N1, B1, kv1_off,
+                             kv1_mod, kv1_base, kv1_rows, scale, accumulate, S(stream));
+}
+
+int b200vton_quantize_kv_e4m3(const void* x, int64_t ldx, int M, int G, int Ng, void* q, int64_t ldq, void* e,
+                              int64_t lde, void* stream) {
+  return vton::quantize_kv_e4m3_impl(x, ldx, M, G, Ng, q, ldq, e, lde, S(stream));
 }
 
 int b200vton_encoder_attention(const void* q, int64_t ldq, const void* k, const void* v, int64_t ldkv, void* out,

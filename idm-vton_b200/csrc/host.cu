@@ -86,7 +86,9 @@ static int encode_tmap_any(CUtensorMap* out, CUtensorMapDataType dtype, const vo
   }
   CUresult r = fn(out, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
                   gstr, gbox, gel, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  swizzle_bytes == 0    ? CU_TENSOR_MAP_SWIZZLE_NONE
+                  : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                        : CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d dims %llu,%llu box %u,%u)", (int)r, rank,
@@ -108,8 +110,8 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
 }
 
 int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box) {
-  return encode_tmap_any(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, nullptr, 128);
+                   const uint32_t* box, int swizzle_bytes) {
+  return encode_tmap_any(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, nullptr, swizzle_bytes);
 }
 
 }  // namespace vton

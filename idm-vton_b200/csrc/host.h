@@ -42,9 +42,10 @@ int encode_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t
 int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                     const uint32_t* box);
 
-// One-byte elements (e4m3 operands of the FP8 linears), SWIZZLE_128B (inner box = 128 elements = 128 B).
+// One-byte elements (e4m3 operands of the FP8 linears), SWIZZLE_128B (inner box = 128 elements = 128 B), or with
+// swizzle_bytes = 0 no swizzle (the FP8 garment K/V tiles and exponents, converted by the attention's producer warps).
 int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box);
+                   const uint32_t* box, int swizzle_bytes = 128);
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 

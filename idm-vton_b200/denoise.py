@@ -13,6 +13,7 @@ import collections
 import torch
 
 from .engine import CIN_PAD, UNetEngine
+from .lib import KV8_GROUP, GarmentKV8
 from .scheduler import DPMSolverMultistepScheduler, _init_step_index, config_getter, solver_order_at
 
 
@@ -255,9 +256,50 @@ def garment_tokens(tryon, hg, wg):
     return [lvl_tokens[b.c] for b in tryon.blocks()]
 
 
-def garment_kv_bytes_per_step(tryon, hg, wg):
-    """Bytes of the hoisted K/V of ONE garment for one denoise step: sum over the try-on blocks of Ng * 2C fp16."""
+def garment_kv_format(tryon):
+    """"fp16" or "fp8": the format the denoisers hold the try-on engine's hoisted garment K/V in (UNetEngine.
+    garment_kv_format; fp16 for an engine that names none)."""
+    return getattr(tryon, "garment_kv_format", "fp16")
+
+
+def new_garment_kv(tryon, rows, ng, blk):
+    """Storage for `rows` rows of one try-on block's hoisted garment K/V in garment_kv_format(tryon): fp16
+    [rows, Ng, 2C], or a GarmentKV8."""
+    if garment_kv_format(tryon) == "fp8":
+        return GarmentKV8.empty(rows, ng, blk.c, tryon.device)
+    return torch.empty((rows, ng, 2 * blk.c), dtype=torch.float16, device=tryon.device)
+
+
+def garment_kv_bytes_per_step(tryon, hg, wg, fmt=None):
+    """Bytes of the hoisted K/V of ONE garment for one denoise step: sum over the try-on blocks of Ng * 2C fp16, or in
+    the "fp8" format (default: the engine's garment_kv_format) Ng * 2C e4m3 plus 2C / 64 int8 exponents per token
+    (Ng rounded up to 16)."""
+    fmt = fmt or garment_kv_format(tryon)
+    if fmt == "fp8":
+        return sum(ng * 2 * b.c + (2 * b.c // KV8_GROUP) * (-(-ng // 16) * 16)
+                   for b, ng in zip(tryon.blocks(), garment_tokens(tryon, hg, wg)))
     return sum(ng * 2 * b.c * 2 for b, ng in zip(tryon.blocks(), garment_tokens(tryon, hg, wg)))
+
+
+def check_garment_kv_held(tryon, what):
+    """FP8 garment K/V exist only as hoisted K/V: refuses, before any launch, a path that computes them in the step."""
+    if garment_kv_format(tryon) != "fp8":
+        return
+    for name in ("b200vton_quantize_kv_e4m3", "b200vton_attention_kv8"):
+        if not tryon.L.has_symbol(name):
+            raise NotImplementedError(f"FP8 garment K/V need {name}, which this library binding does not export")
+    if what is not None:
+        raise NotImplementedError(f"garment K/V precision 'fp8' with {what}: only hoisted garment K/V are held in the "
+                                  "FP8 format (the garment K/V of this path are computed inside the step)")
+
+
+def kv_map(kv, fn):
+    """fn applied to a block's hoisted garment K/V: the fp16 tensor, or both parts of a GarmentKV8 (rows first)."""
+    return kv.map(fn) if isinstance(kv, GarmentKV8) else fn(kv)
+
+
+def kv_parts(kv):
+    return tuple(kv) if isinstance(kv, GarmentKV8) else (kv,)
 
 
 def hoisted_garment_kv(tryon, garment, x_g, ctx_g, t_table, t0, t1, chunk, out):
@@ -277,8 +319,9 @@ def hoisted_garment_kv(tryon, garment, x_g, ctx_g, t_table, t0, t1, chunk, out):
         feats = []
         garment.forward(x_big, garment.time_embedding(t_rows, n * Bg), ctx_big, collect=feats)
         for i, (blk, f) in enumerate(zip(blocks, feats)):
-            tryon.garment_kv(blk, f, out=out[i][c0 * Bg:(c0 + n) * Bg])
+            tryon.garment_kv(blk, f, out=kv_map(out[i], lambda t: t[c0 * Bg:(c0 + n) * Bg]))
         del feats, x_big, ctx_big
+    tryon.release_kv_scratch()
 
 
 def default_garment_chunk(Bg):
@@ -290,7 +333,8 @@ def default_garment_chunk(Bg):
 class GarmentKVCache:
     """LRU cache of hoisted garment K/V across requests (SURVEY.md 8f item 4). One entry = the K/V of ONE garment for every
     denoise step and every try-on block ([T, Ng, 2C] fp16 per block: 9.44 GB of K and V at 768x1024 / 30 steps, computed
-    from the shapes), keyed by the caller's garment id plus everything the values depend on (timestep list, the garment's latent size). A hit replaces the
+    from the shapes; a GarmentKV8 per block in the "fp8" format, 4.79 GB), keyed by the caller's garment id plus
+    everything the values depend on (timestep list, the garment's latent size, the format). A hit replaces the
     garment's T garment-UNet passes by device-to-device copies (~2 ms)."""
 
     def __init__(self, max_bytes=16 << 30):   # beside 11 GB of weights and the step's K/V on an 80 GB H100
@@ -309,7 +353,7 @@ class GarmentKVCache:
         return e[0]
 
     def put(self, key, tensors):
-        n = sum(t.numel() * t.element_size() for t in tensors)
+        n = sum(p.numel() * p.element_size() for t in tensors for p in kv_parts(t))
         if n > self.max_bytes:
             return
         if key in self.entries:
@@ -479,9 +523,10 @@ class TryOnDenoiser(_CapturedStep):
             if tuple(t.shape[-2:]) != (h, w):
                 raise ValueError(f"{name} has spatial size {tuple(t.shape[-2:])}, the latents {(h, w)}: the try-on UNet "
                                  "input concatenates them along channels")
+        check_garment_kv_held(self.tryon, None if self.hoist_garment else "TryOnDenoiser(hoist_garment=False)")
         rescale = bool(do_cfg) and guidance_rescale > 0
         key = (B, Bt, Bg, h, w, hg, wg, bool(do_cfg), rescale, tuple(prompt_embeds.shape), tuple(image_embeds.shape),
-               tuple(text_embeds_cloth.shape))
+               tuple(text_embeds_cloth.shape), garment_kv_format(self.tryon))
         fresh = key != getattr(self, "_key", None)
         self._key = key
         self.B, self.Bt, self.Bg, self.h, self.w = B, Bt, Bg, h, w
@@ -536,7 +581,8 @@ class TryOnDenoiser(_CapturedStep):
                 # not handed out + the K/V buffers of the previous request, which are overwritten in place
                 free, _ = torch.cuda.mem_get_info(self.device)
                 cached = torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
-                held = sum(g.numel() * 2 for g in self.gkv_all) if self.gkv_all is not None else 0
+                held = sum(p.numel() * p.element_size() for g in self.gkv_all for p in kv_parts(g)) \
+                    if self.gkv_all is not None else 0
                 budget = int(0.6 * (free + cached + held))
             per_step = self.kv_bytes_per_step()
             if per_step * T > budget:
@@ -546,25 +592,27 @@ class TryOnDenoiser(_CapturedStep):
         if self.hoist_garment:
             use_cache = cache is not None and garment_keys is not None and len(garment_keys) == self.Bg and self.window == T
             if use_cache:
-                sig = (tuple(float(t) for t in timesteps), self.hg, self.wg)
+                sig = (tuple(float(t) for t in timesteps), self.hg, self.wg, garment_kv_format(self.tryon))
                 full = [(k, sig) for k in garment_keys]
                 hit = [cache.get(k) for k in full]
                 if all(e is not None for e in hit):
-                    if self.gkv_all is None or self.gkv_all[0].shape[0] != T * self.Bg:
+                    if self.gkv_all is None or kv_parts(self.gkv_all[0])[0].shape[0] != T * self.Bg:
                         # first request of this shape (prepare() dropped the static buffers): allocate them from the cached
                         # entries' geometry instead of re-running the garment passes; the step graph is captured afterwards
-                        self.gkv_all = [torch.empty((T * self.Bg, *src.shape[1:]), dtype=src.dtype, device=self.device)
-                                        for src in hit[0]]
+                        self.gkv_all = [kv_map(src, lambda t: torch.empty((T * self.Bg, *t.shape[1:]), dtype=t.dtype,
+                                                                          device=self.device)) for src in hit[0]]
                     for g, e in enumerate(hit):                         # timestep-major rows: row = t * Bg + g
                         for dst, src in zip(self.gkv_all, e):
-                            dst.view(T, self.Bg, *dst.shape[1:])[:, g].copy_(src)
+                            for d, s_ in zip(kv_parts(dst), kv_parts(src)):
+                                d.view(T, self.Bg, *d.shape[1:])[:, g].copy_(s_)
                     self.win_start = 0
                     return
             self.precompute_garment(0)
             if use_cache:
                 for g, k in enumerate(full):
                     if k not in cache.entries:
-                        cache.put(k, [t.view(T, self.Bg, *t.shape[1:])[:, g].clone() for t in self.gkv_all])
+                        cache.put(k, [kv_map(kv, lambda t: t.view(T, self.Bg, *t.shape[1:])[:, g].clone())
+                                      for kv in self.gkv_all])
 
     @property
     def garment_chunk(self):
@@ -575,8 +623,9 @@ class TryOnDenoiser(_CapturedStep):
         return default_garment_chunk(getattr(self, "Bg", 1))
 
     def kv_bytes_per_step(self):
-        """Bytes of garment K/V one denoise step keeps resident: sum over the try-on blocks of Bg * Ng * 2C fp16, Ng = the
-        garment's tokens at the block's level (from the cloth latents' size)."""
+        """Bytes of garment K/V one denoise step keeps resident: sum over the try-on blocks of Bg * Ng * 2C fp16 (or the
+        FP8 format's bytes, garment_kv_bytes_per_step), Ng = the garment's tokens at the block's level (from the cloth
+        latents' size)."""
         return self.Bg * garment_kv_bytes_per_step(self.tryon, self.hg, self.wg)
 
     def precompute_garment(self, win_start=0):
@@ -591,14 +640,14 @@ class TryOnDenoiser(_CapturedStep):
         T = min(self.window, T_all - win_start)
         rows = min(self.window, T_all) * Bg
         gkv = self.gkv_all            # buffers of an earlier same-shaped request are overwritten in place
-        if gkv is not None and gkv[0].shape[0] != rows:
+        if gkv is not None and kv_parts(gkv[0])[0].shape[0] != rows:
             gkv = None
         self.gkv_all = None
         if gkv is None:
-            gkv = [torch.empty((rows, ng, 2 * b.c), dtype=torch.float16, device=self.device)
+            gkv = [new_garment_kv(self.tryon, rows, ng, b)
                    for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, self.hg, self.wg))]
         hoisted_garment_kv(self.tryon, self.garment, self.x_g, self.ctx_g, self.t_table, win_start, win_start + T,
-                           self.garment_chunk, [g[:T * Bg] for g in gkv])
+                           self.garment_chunk, [kv_map(g, lambda t: t[:T * Bg]) for g in gkv])
         self.gkv_all = gkv
         self.win_start = win_start
 
@@ -638,7 +687,7 @@ class SlotDenoiser(_CapturedStep):
       * pages=None (default): the garment UNet runs inside the step at batch S with per-slot timesteps, and the garment
         features of slot s are streamed into try-on rows s / S + s. Nothing is hoisted.
       * pages=P (pool mode, P >= S): the hoisted garment K/V of whole garments live in a pool of P pages, one tensor
-        [P*T, Ng, 2C] per try-on block (page p = rows p*T .. p*T + T - 1, so one TMA map per block covers every page and
+        [P*T, Ng, 2C] per try-on block (a GarmentKV8 of P*T rows in the "fp8" garment K/V format) (page p = rows p*T .. p*T + T - 1, so one TMA map per block covers every page and
         the captured graph stays valid while pages are refilled). fill_page runs the T garment passes of one garment
         alone (Bg = 1, TryOnDenoiser's default chunking, hoisted_garment_kv), so a page's bits depend only on the garment
         and the timesteps. The step is the try-on UNet only: slot s reads row page(s)*T + step(s) of the pool through
@@ -681,6 +730,10 @@ class SlotDenoiser(_CapturedStep):
             names.append("b200vton_attention_rows")
         return names
 
+    def _check_kv_format(self):
+        check_garment_kv_held(self.tryon, "continuous batching without a garment K/V pool (pages=None)"
+                              if self.P is None else None)
+
     def configure(self, scheduler, timesteps, h, w, guidance_scale=2.0, do_cfg=True, eta=0.0, guidance_rescale=0.0):
         """Per-step tables of the run (one scheduler, one step count for every request) and the static buffers of a
         person latent size h x w (the garment has the same size). Raises before any launch when the library lacks a
@@ -690,6 +743,7 @@ class SlotDenoiser(_CapturedStep):
             raise NotImplementedError("guidance_rescale > 0 is not supported by continuous batching: the rescale kernel "
                                       "reads one coefficient row for the whole batch")
         plan = step_plan(scheduler, timesteps, guidance_scale, eta=eta)    # row T: idle slots
+        self._check_kv_format()
         for name in self._needs(plan.kind):
             if not self.L.has_symbol(name):
                 raise NotImplementedError(f"continuous batching needs {name}, which this library binding does not export")
@@ -713,6 +767,7 @@ class SlotDenoiser(_CapturedStep):
         for name in self._needs("mixed"):
             if not self.L.has_symbol(name):
                 raise NotImplementedError(f"sampling presets need {name}, which this library binding does not export")
+        self._check_kv_format()
         f32 = torch.float32
         idle = plans[0].kind
         self.base, n = [], 0
@@ -740,7 +795,8 @@ class SlotDenoiser(_CapturedStep):
         self.do_cfg, self.h, self.w = bool(do_cfg), h, w
         S = self.S
         self.Bt = 2 * S if do_cfg else S
-        key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T_page))
+        key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T_page,
+                                                                               garment_kv_format(self.tryon)))
         if key != self._key:
             self._key = key
             self.ctx_t = self.ctx_g = self.aug = None
@@ -756,7 +812,7 @@ class SlotDenoiser(_CapturedStep):
                 # allocated once (the old pool is released first); every page is written by fill_page before a slot's
                 # row names it
                 self.x_g = self.t_g = self.pool = None
-                self.pool = [torch.empty((self.P * self.T_page, ng, 2 * b.c), dtype=f16, device=dev)
+                self.pool = [new_garment_kv(self.tryon, self.P * self.T_page, ng, b)
                              for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, h, w))]
                 self.rows = torch.full((S,), -1, dtype=torch.int32, device=dev)
                 self.page = [None] * S
@@ -828,7 +884,7 @@ class SlotDenoiser(_CapturedStep):
             self.L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), x_g, c_off=0)
             ctx_g = self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16))
             hoisted_garment_kv(self.tryon, self.garment, x_g, ctx_g, t_table, 0, T, self.garment_chunk,
-                               [g[p * Tp:p * Tp + T] for g in self.pool])
+                               [kv_map(g, lambda t: t[p * Tp:p * Tp + T]) for g in self.pool])
 
     def _rows(self, s):
         return (s, self.S + s) if self.do_cfg else (s,)

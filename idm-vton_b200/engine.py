@@ -110,6 +110,10 @@ class UNetEngine:
         self.ip_tokens = cfg["ip_tokens"] if kind == "tryon" else 0
         self.ip_scales = dict(ip_scales or {})
         self.fp8 = bool(fp8)
+        # format of the hoisted garment K/V the denoisers keep for this (try-on) UNet: "fp16" or "fp8" (lib.GarmentKV8);
+        # set by UNet2DConditionModel.set_garment_kv_precision
+        self.garment_kv_format = "fp16"
+        self._kv_scratch = None
         if self.fp8:
             for name in ("b200vton_layernorm_e4m3", "b200vton_gemm_e4m3"):
                 if not lib.has_symbol(name):
@@ -310,11 +314,24 @@ class UNetEngine:
         assert x1 is None
         return L.conv3x3(h, r.w2, bias=r.b2, residual=x0)
 
+    def release_kv_scratch(self):
+        """Drops the fp16 scratch of garment_kv's FP8 route (called after a run of hoisted passes, so the memory goes back
+        to the allocator that the K/V budgets count as available)."""
+        self._kv_scratch = None
+
     def garment_kv(self, blk, gfeat, out=None):
         """K/V of garment tokens as the TRY-ON UNet sees them: attn1.to_k / to_v applied to the garment UNet's
         post-norm1 feature (src/attentionhacked_tryon.py:334 + ip_adapter/attention_processor.py:247-248).
-        gfeat [n, Ng, C] -> [n, Ng, 2C] = [K | V]."""
+        gfeat [n, Ng, C] -> [n, Ng, 2C] = [K | V]. out may be a lib.GarmentKV8: the fp16 K/V then go to a scratch
+        buffer reused across calls and are quantized into it (the same GEMM, so the same fp16 bits before the rule)."""
         n, ng, C = gfeat.shape
+        if isinstance(out, self.L.GarmentKV8):
+            need = n * ng * 2 * C
+            if self._kv_scratch is None or self._kv_scratch.numel() < need:
+                self._kv_scratch = None
+                self._kv_scratch = torch.empty(need, dtype=torch.float16, device=self.device)
+            kv = self.garment_kv(blk, gfeat, out=self._kv_scratch[:need].view(n, ng, 2 * C))
+            return self.L.quantize_kv_e4m3(kv, out)
         o2 = None if out is None else out.view(n * ng, 2 * C)
         return self.L.gemm(gfeat.reshape(n * ng, C), blk.wqkv[C:], out=o2).view(n, ng, 2 * C)
 
@@ -323,7 +340,7 @@ class UNetEngine:
         (reference-format features through the module seam) or None (garment UNet). gkv_pre = (kv [T*Bg,Ng,2C],
         n_garments, step_base int32 device scalar): garment K/V precomputed for all denoise steps; or (pool [P*T,Ng,2C],
         rows int32 device [B - n_persons]): a pool of hoisted K/V pages, person sample j reading row rows[j] (negative:
-        zero K/V, an idle slot)."""
+        zero K/V, an idle slot). The hoisted K/V may be a lib.GarmentKV8 (FP8 garment K/V) in either form."""
         L = self.L
         C, H = blk.c, blk.heads
         f8 = blk.fp8
@@ -345,11 +362,17 @@ class UNetEngine:
         q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
         if gkv_pre is not None and len(gkv_pre) == 2:
             pool, rows = gkv_pre
-            a = L.attention_rows(q, k, v, pool[..., :C], pool[..., C:], rows, kv1_off=n_persons, heads=H)
+            if isinstance(pool, L.GarmentKV8):
+                a = L.attention_kv8(q, k, v, pool, kv1_off=n_persons, heads=H, kv1_rows=rows)
+            else:
+                a = L.attention_rows(q, k, v, pool[..., :C], pool[..., C:], rows, kv1_off=n_persons, heads=H)
         elif gkv_pre is not None:
             kv_all, n_g, base = gkv_pre
-            a = L.attention(q, k, v, kv_all[..., :C], kv_all[..., C:], kv1_off=n_persons, heads=H, kv1_mod=n_g,
-                            kv1_base=base)
+            if isinstance(kv_all, L.GarmentKV8):
+                a = L.attention_kv8(q, k, v, kv_all, kv1_off=n_persons, heads=H, kv1_mod=n_g, kv1_base=base)
+            else:
+                a = L.attention(q, k, v, kv_all[..., :C], kv_all[..., C:], kv1_off=n_persons, heads=H, kv1_mod=n_g,
+                                kv1_base=base)
         elif gfeat is None:
             a = L.attention(q, k, v, heads=H)
         else:

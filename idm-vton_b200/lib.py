@@ -48,8 +48,8 @@ SIGNATURES = {
 }
 
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
-# step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears and
-# the per-sample-row attention of its pool mode.
+# step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears,
+# the per-sample-row attention of its pool mode and the FP8 garment K/V (quantizer and attention).
 # `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
@@ -60,6 +60,9 @@ OPTIONAL_SIGNATURES = {
     "b200vton_attention_rows": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp,
                                 _f, _i, _vp],
     "b200vton_cfg_step_mixed_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp],
+    "b200vton_quantize_kv_e4m3": [_vp, _i64, _i, _i, _i, _vp, _i64, _vp, _i64, _vp],
+    "b200vton_attention_kv8": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i,
+                               _i, _i, _vp, _vp, _f, _i, _vp],
 }
 _present = set()
 
@@ -266,6 +269,82 @@ def attention_rows(q, k0, v0, k1, v1, kv1_rows, kv1_off=0, heads=None, scale=Non
     rc = fn(_p(q), q.stride(1), _p(k0), _p(v0), k0.stride(1), _p(k1), _p(v1), ld1, _p(out), out.stride(1), B, heads, Nq,
             N0, n1, B1, kv1_off, _p(kv1_rows), float(scale), int(accumulate), _stream())
     _check(rc, "b200vton_attention_rows")
+    return out
+
+
+KV8_GROUP = 64     # columns per exponent of the FP8 garment K/V (one head of K or of V)
+
+
+class GarmentKV8(tuple):
+    """Hoisted garment K/V in the FP8 format (include/b200vton.h, b200vton_quantize_kv_e4m3): (q, e) with q e4m3
+    [rows, Ng, 2C] and e int8 [rows, 2H, Ng_pad] (Ng_pad = Ng rounded up to 16). Both have `rows` first, so a row range,
+    a view or a copy of the pair applies to both (map)."""
+
+    def __new__(cls, q, e):
+        return super().__new__(cls, (q, e))
+
+    q = property(lambda self: self[0])
+    e = property(lambda self: self[1])
+
+    @staticmethod
+    def empty(rows, ng, c, device):
+        """Storage for `rows` rows of Ng tokens and C channels (2C / 64 exponent groups per token)."""
+        return GarmentKV8(torch.empty((rows, ng, 2 * c), dtype=E4M3, device=device),
+                          torch.empty((rows, 2 * c // KV8_GROUP, -(-ng // 16) * 16), dtype=torch.int8, device=device))
+
+    def map(self, fn):
+        return GarmentKV8(fn(self[0]), fn(self[1]))
+
+
+def quantize_kv_e4m3(x, out):
+    """x: fp16 [rows, Ng, 2C] (contiguous last dim, rows and tokens may be strided as one [rows*Ng, 2C] matrix) ->
+    out = GarmentKV8 of the same rows, by the rule of include/b200vton.h (bit-identical)."""
+    fn = _optional("b200vton_quantize_kv_e4m3")
+    _f16(x, "x")
+    rows, ng, c2 = x.shape
+    q, e = out
+    if q.dtype != E4M3 or e.dtype != torch.int8 or tuple(q.shape) != (rows, ng, c2) or \
+            tuple(e.shape[:2]) != (rows, c2 // KV8_GROUP) or e.shape[2] < ng or not e.is_contiguous():
+        raise ValueError(f"quantize_kv_e4m3: out must be (e4m3 {(rows, ng, c2)}, contiguous int8 "
+                         f"{(rows, c2 // KV8_GROUP)} x >= {ng}), got {q.dtype} {tuple(q.shape)}, {e.dtype} "
+                         f"{tuple(e.shape)}")
+    x2, q2 = x.reshape(rows * ng, c2), q.view(rows * ng, c2)     # a view: the kernel must write the caller's storage
+    assert x2.stride(1) == 1 and q2.stride(1) == 1
+    rc = fn(_p(x2), x2.stride(0), rows * ng, c2 // KV8_GROUP, ng, _p(q2), q2.stride(0), _p(e), e.shape[2], _stream())
+    _check(rc, "b200vton_quantize_kv_e4m3")
+    return out
+
+
+def attention_kv8(q, k0, v0, kv1, kv1_off=0, heads=None, scale=None, accumulate=False, out=None, kv1_mod=0,
+                  kv1_base=None, kv1_rows=None):
+    """attention (or, with kv1_rows, attention_rows) with segment 1 = kv1, a GarmentKV8 of [B1, N1, 2C] garment K/V
+    (K = columns [0, C), V = [C, 2C), C = heads * 64): the result of those calls on kv1 dequantized, bit for bit."""
+    fn = _optional("b200vton_attention_kv8")
+    B, Nq = q.shape[0], q.shape[1]
+    N0 = k0.shape[1]
+    H = heads
+    C = H * 64
+    assert q.stride(2) == 1 and k0.stride(2) == 1 and v0.stride(2) == 1
+    assert q.stride(0) == Nq * q.stride(1) and k0.stride(0) == N0 * k0.stride(1) and v0.stride() == k0.stride()
+    kq, e = kv1
+    B1, n1 = kq.shape[0], kq.shape[1]
+    if kq.dtype != E4M3 or kq.shape[2] != 2 * C or kq.stride(2) != 1 or kq.stride(0) != n1 * kq.stride(1):
+        raise ValueError(f"attention_kv8: kv1.q must be e4m3 [B1, N1, {2 * C}] rows, got {kq.dtype} {tuple(kq.shape)}")
+    if e.dtype != torch.int8 or tuple(e.shape[:2]) != (B1, 2 * H) or not e.is_contiguous():
+        raise ValueError(f"attention_kv8: kv1.e must be contiguous int8 [{B1}, {2 * H}, Ng_pad], got {e.dtype} "
+                         f"{tuple(e.shape)}")
+    if kv1_rows is not None and (kv1_rows.dtype != torch.int32 or not kv1_rows.is_cuda or
+                                 not kv1_rows.is_contiguous() or kv1_rows.numel() != B - kv1_off):
+        raise ValueError(f"attention_kv8: kv1_rows must be a contiguous CUDA int32 tensor of B - kv1_off = "
+                         f"{B - kv1_off} entries, got {kv1_rows.dtype} {tuple(kv1_rows.shape)} on {kv1_rows.device}")
+    if scale is None:
+        scale = 64 ** -0.5
+    if out is None:
+        out = torch.empty((B, Nq, C), dtype=torch.float16, device=q.device)
+    rc = fn(_p(q), q.stride(1), _p(k0), _p(v0), k0.stride(1), _p(kq), _p(kq[..., C:]), kq.stride(1), _p(e), e.shape[2],
+            _p(out), out.stride(1), B, H, Nq, N0, n1, B1, kv1_off, kv1_mod, _p(kv1_base), _p(kv1_rows), float(scale),
+            int(accumulate), _stream())
+    _check(rc, "b200vton_attention_kv8")
     return out
 
 

@@ -141,6 +141,17 @@ class StableDiffusionXLInpaintPipeline:
         if self.garment_cache is not None:
             self.garment_cache.clear()
 
+    def set_garment_kv_precision(self, precision):
+        """"fp16" (default) or "fp8" for the hoisted garment K/V of the try-on UNet (INTEGRATION.md, "FP8 garment K/V"):
+        e4m3 with a power-of-two exponent per token and head, about half the bytes. A change drops the denoiser with its
+        held K/V and graphs, and the garment K/V cached in the other format."""
+        prev = self.unet.garment_kv_precision
+        self.unet.set_garment_kv_precision(precision)
+        if precision != prev:
+            self._denoiser = None
+            if self.garment_cache is not None:
+                self.garment_cache.clear()
+
     def register_to_config(self, **kw):
         for k, v in kw.items():
             setattr(self.config, k, v)

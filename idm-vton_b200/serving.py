@@ -482,8 +482,16 @@ class ContinuousTryOnServer:
         free = [s for s, e in enumerate(self.slots) if e is None]
         if not free or not self.waiting:
             return
+        fmt = getattr(self.pipe.unet, "garment_kv_precision", "fp16")
+        if getattr(self, "_configured", False) and fmt != self._kv_format:
+            # the pipe's garment K/V precision changed: the pool, its page count and the page table are in the old format
+            if any(e is not None for e in self.slots):
+                raise RuntimeError(f"the pipeline's garment K/V precision changed to {fmt!r} while requests run in "
+                                   f"{self._kv_format!r}: change it when the server is idle")
+            self.den, self._configured = None, False
         if not getattr(self, "_configured", False):
             self._configure()
+            self._kv_format = fmt
         device, dtype = self.pipe._execution_device, self.pipe.unet.dtype
         for s in free:
             if not self.waiting:

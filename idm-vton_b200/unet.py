@@ -398,6 +398,28 @@ class UNet2DConditionModel(_UNetBase):
 
     def __init__(self, cfg=None, state_dict=None, device="cpu", dtype=torch.float16):
         super().__init__(cfg or SDXL_TRYON, state_dict, device, dtype)
+        self._garment_kv_precision = "fp16"
+
+    GARMENT_KV_PRECISIONS = ("fp16", "fp8")
+
+    @property
+    def garment_kv_precision(self):
+        return self._garment_kv_precision
+
+    def set_garment_kv_precision(self, precision):
+        """"fp16" (default) or "fp8": the format the denoisers hold the hoisted garment K/V of this UNet in (e4m3 with
+        one power-of-two exponent per token and head, INTEGRATION.md "FP8 garment K/V"). The weights are not re-packed;
+        a denoiser allocates its garment K/V in the new format at its next prepare / configure."""
+        if precision not in self.GARMENT_KV_PRECISIONS:
+            raise ValueError(f"garment K/V precision must be one of {self.GARMENT_KV_PRECISIONS}, got {precision!r}")
+        self._garment_kv_precision = precision
+        if self._engine is not None:
+            self._engine.garment_kv_format = precision
+
+    def engine(self):
+        eng = super().engine()
+        eng.garment_kv_format = self._garment_kv_precision
+        return eng
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, timestep_cond=None,
@@ -416,6 +438,10 @@ class UNet2DConditionModel(_UNetBase):
                              "(src/unet_hacked_tryon.py:1174-1242)")
         if garment_features is None:
             raise ValueError("garment_features is required (src/attentionhacked_tryon.py:334)")
+        if self._garment_kv_precision == "fp8":
+            raise NotImplementedError("garment K/V precision 'fp8' with the module forward's reference-format "
+                                      "garment_features: only hoisted garment K/V (the engine pipeline's denoiser) are "
+                                      "held in the FP8 format")
         eng = self.engine()
         L = self._lib
         f16 = torch.float16

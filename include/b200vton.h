@@ -97,6 +97,30 @@ int b200vton_attention_rows(const void* q, int64_t ldq, const void* k0, const vo
                             const void* v1, int64_t ldkv1, void* out, int64_t ldo, int B, int H, int Nq, int N0, int N1,
                             int B1, int kv1_off, const void* kv1_rows, float scale, int accumulate, void* stream);
 
+/* FP8 garment K/V (opt-in, set_garment_kv_precision("fp8"); INTEGRATION.md, "FP8 garment K/V"). The format of the
+ * hoisted garment K/V [rows, Ng, 2C] (K in columns [0, C), V in [C, 2C)): per token and per group of 64 columns (group
+ * g < H = head g of K, group H + g = head g of V), with amax = max |x| over the group in fp32,
+ *   e = 0 when amax == 0, else the smallest integer with amax <= 448 * 2^e, clamped to e >= -24;
+ *   q = e4m3_rn_satfinite(x * 2^-e) (exact product, |.| <= 448);   x' = fp16_rn(float(q) * 2^e).
+ * q: [rows, Ng, 2C] e4m3; e: int8 [rows, 2H, lde] (group-major, lde >= Ng a multiple of 16, entries >= Ng are 0).
+ *
+ * b200vton_quantize_kv_e4m3: x fp16 [M, G*64] (row stride ldx, a multiple of 8; 16-byte aligned), M = rows * Ng ->
+ * q e4m3 [M, ldq] (ldq a multiple of 8; 8-byte aligned) and e int8 [rows, G, lde] (lde >= Ng; the padding is written 0).
+ * Bit-identical to the rule above. */
+int b200vton_quantize_kv_e4m3(const void* x, int64_t ldx, int M, int G, int Ng, void* q, int64_t ldq, void* e,
+                              int64_t lde, void* stream);
+
+/* b200vton_attention with segment 1 in the FP8 garment K/V format: k1 / v1 are e4m3 [B1, N1, *] views (row stride ldkv1
+ * BYTES, a multiple of 16; 16-byte aligned), e1 the int8 exponents [B1, 2H, lde1] of the same rows (lde1 a multiple of
+ * 16, >= N1; 16-byte aligned). The kernel dequantizes each tile by the rule (exact: x' = fp16(q) * fp16(2^e) in one
+ * rounding), so the result is b200vton_attention's on the dequantized K/V, bit for bit. kv1_rows (device int32
+ * [B - kv1_off], or NULL) selects segment-1 rows as in b200vton_attention_rows and replaces kv1_mod / kv1_base; without
+ * it, kv1_mod / kv1_base as in b200vton_attention. Needs N1 > 0, B1 > 0 and 0 <= kv1_off < B; head_dim 64. */
+int b200vton_attention_kv8(const void* q, int64_t ldq, const void* k0, const void* v0, int64_t ldkv0, const void* k1,
+                           const void* v1, int64_t ldkv1, const void* e1, int64_t lde1, void* out, int64_t ldo, int B,
+                           int H, int Nq, int N0, int N1, int B1, int kv1_off, int kv1_mod, const void* kv1_base,
+                           const void* kv1_rows, float scale, int accumulate, void* stream);
+
 /* Decoupled cross-attention (attn2 of every transformer block) in one launch:
  *   out = fp16( fp16(softmax(Q Kt^T * scale) Vt) + fp16(ip_scale * fp16(softmax(Q Ki^T * scale) Vi)) ),  head_dim 64,
  * Kt/Vt = [B, Nt <= 80, *] the text tokens (attn2.to_k / to_v), Ki/Vi = [B, Ni <= 16, *] the IP-Adapter image tokens

@@ -18,7 +18,11 @@ full occupancy, measured first. Prints one JSON line with, per mode:
 and the step time at full occupancy (the default continuous step graph and the pool step graph at S slots) against the
 batch-mode step at batch S with one garment plus its hoisted garment passes per step; the time of one page fill (a
 miss); the card's name and power limit, read in the same run.
-Usage: python scripts/continuous_timing.py [--slots 4] [--requests 32] [--garments 8] [--rounds 2] [--kv-gb 40]"""
+--garment-kv fp8 runs batch mode and pool mode with the pipeline's FP8 garment K/V (pipe.set_garment_kv_precision):
+batch mode's cache entries and the pool's pages are then about half the size. The default continuous mode holds no
+garment K/V and refuses the format, so it only sets the arrival rate, as in fp16.
+Usage: python scripts/continuous_timing.py [--slots 4] [--requests 32] [--garments 8] [--rounds 2] [--kv-gb 40]
+       [--garment-kv fp16|fp8]"""
 import argparse
 import json
 import os
@@ -93,6 +97,8 @@ def main():
     ap.add_argument("--load", type=float, default=0.9)
     ap.add_argument("--kv-gb", type=float, default=40,
                     help="garment K/V budget of batch mode's cache and of the pool (GB, 1e9 bytes)")
+    ap.add_argument("--garment-kv", default="fp16", choices=("fp16", "fp8"), dest="garment_kv",
+                    help="precision of the hoisted garment K/V (cache entries and pool pages)")
     args = ap.parse_args()
     kv_bytes = int(args.kv_gb * 1e9)
     from idm_vton_b200 import lib as L
@@ -107,7 +113,8 @@ def main():
     unet, unet_enc, _ = bench.build_components(dev, 0, 1, lambda m: None)
     pipe = bench.make_pipeline(unet, unet_enc, dev)
     out = {"card": card(), "config": f"768x1024, DDPM {T} steps, guidance 2.0, random SDXL weights, S = {S}, "
-                                      f"{args.requests} requests over {args.garments} garments"}
+                                      f"{args.requests} requests over {args.garments} garments, "
+                                      f"garment K/V {args.garment_kv}"}
     ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
 
     # the step at full occupancy: continuous (S slots, per-slot garment passes) vs batch (S persons, one garment,
@@ -125,6 +132,9 @@ def main():
     cont_step = e0.elapsed_time(e1) / 10
     del cont
     torch.cuda.empty_cache()
+    # the garment K/V format from here on (the default continuous server above, which holds no garment K/V, sets the
+    # arrival rate in either format; with fp8 it is not a mode of the trace: it refuses FP8 garment K/V)
+    pipe.set_garment_kv_precision(args.garment_kv)
     # the same for pool mode (S garments filled at admission), then the time of one page fill
     pool = ContinuousTryOnServer(pipe, height=H, width=W, slots=S, num_inference_steps=T, guidance_scale=2.0, seed=7,
                                  garment_kv_bytes=kv_bytes)
@@ -189,6 +199,8 @@ def main():
         "continuous_pool": lambda: ContinuousTryOnServer(pipe, height=H, width=W, slots=S, num_inference_steps=T,
                                                          guidance_scale=2.0, seed=7, garment_kv_bytes=kv_bytes),
     }
+    if args.garment_kv == "fp8":
+        del modes["continuous"]
     import gc
 
     def fresh(name):
