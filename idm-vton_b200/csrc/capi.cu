@@ -79,6 +79,9 @@ int cfg_solver_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, c
 int cfg_mixed_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, const void* latents, const void* noise,
                         void* x0_prev, const void* coef, int coef_stride, const void* kinds, int do_cfg, void* out,
                         cudaStream_t stream);
+int resample_u8_impl(const b200vton_resample_desc* descs, const void* descs_dev, int n, const int32_t* tables,
+                     long long table_len, void* workspace, long long workspace_bytes, cudaStream_t stream);
+int paste_u8_impl(const b200vton_paste_desc* descs, const void* descs_dev, int n, cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
@@ -299,6 +302,14 @@ int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_ch
 }
 int b200vton_postprocess_image(const void* x, int nhwc, int B, int H, int W, void* out_pt, void* out_u8, void* stream) {
   return vton::postprocess_impl(x, nhwc, B, H, W, out_pt, out_u8, S(stream));
+}
+
+int b200vton_resample_u8(const b200vton_resample_desc* descs, const void* descs_dev, int n, const int32_t* tables,
+                         int64_t table_len, void* workspace, int64_t workspace_bytes, void* stream) {
+  return vton::resample_u8_impl(descs, descs_dev, n, tables, table_len, workspace, workspace_bytes, S(stream));
+}
+int b200vton_paste_u8(const b200vton_paste_desc* descs, const void* descs_dev, int n, void* stream) {
+  return vton::paste_u8_impl(descs, descs_dev, n, S(stream));
 }
 
 }  // extern "C"

@@ -49,7 +49,8 @@ SIGNATURES = {
 
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
 # step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears,
-# the per-sample-row attention of its pool mode and the FP8 garment K/V (quantizer and attention).
+# the per-sample-row attention of its pool mode, the FP8 garment K/V (quantizer and attention) and the full-resolution
+# photo kernels (resampler and paste-back).
 # `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
@@ -63,6 +64,8 @@ OPTIONAL_SIGNATURES = {
     "b200vton_quantize_kv_e4m3": [_vp, _i64, _i, _i, _i, _vp, _i64, _vp, _i64, _vp],
     "b200vton_attention_kv8": [_vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i,
                                _i, _i, _vp, _vp, _f, _i, _vp],
+    "b200vton_resample_u8": [_vp, _vp, _i, _vp, _i64, _vp, _i64, _vp],
+    "b200vton_paste_u8": [_vp, _vp, _i, _vp],
 }
 _present = set()
 
@@ -871,3 +874,53 @@ def cfg_step_mixed_rows(eps, latents, noise, coef, kinds, x0_prev, do_cfg=True, 
             int(do_cfg), _p(out), _stream())
     _check(rc, "b200vton_cfg_step_mixed_rows")
     return out
+
+
+class ResampleDesc(ctypes.Structure):
+    """b200vton_resample_desc (include/b200vton.h): one crop to resample."""
+    _fields_ = [("src", _vp), ("src_pitch", _i64), ("src_w", _c.c_int32), ("src_h", _c.c_int32),
+                ("crop_x", _c.c_int32), ("crop_y", _c.c_int32), ("crop_w", _c.c_int32), ("crop_h", _c.c_int32),
+                ("dst", _vp), ("dst_pitch", _i64), ("out_f32", _vp), ("out_w", _c.c_int32), ("out_h", _c.c_int32),
+                ("channels", _c.c_int32), ("f32_mode", _c.c_int32),
+                ("bounds_x", _c.c_int32), ("coefs_x", _c.c_int32), ("ksize_x", _c.c_int32), ("need_x", _c.c_int32),
+                ("bounds_y", _c.c_int32), ("coefs_y", _c.c_int32), ("ksize_y", _c.c_int32), ("need_y", _c.c_int32),
+                ("tmp_offset", _i64), ("tmp_first", _c.c_int32), ("tmp_rows", _c.c_int32)]
+
+
+class PasteDesc(ctypes.Structure):
+    """b200vton_paste_desc (include/b200vton.h): one photo's paste-back."""
+    _fields_ = [("photo", _vp), ("photo_pitch", _i64), ("dst", _vp), ("dst_pitch", _i64), ("image", _vp),
+                ("image_pitch", _i64), ("mask", _vp), ("mask_pitch", _i64),
+                ("width", _c.c_int32), ("height", _c.c_int32), ("box_x", _c.c_int32), ("box_y", _c.c_int32),
+                ("box_w", _c.c_int32), ("box_h", _c.c_int32), ("mask_x", _c.c_int32), ("mask_y", _c.c_int32),
+                ("mask_w", _c.c_int32), ("mask_h", _c.c_int32)]
+
+
+def _descs_to_device(descs, device):
+    """A ctypes array of descriptors -> (the array, its device copy) through pinned memory (no host sync; the caching
+    host allocator keeps the staging block until the copy has run)."""
+    host = torch.frombuffer(bytearray(descs), dtype=torch.uint8).pin_memory()
+    return host.to(device, non_blocking=True)
+
+
+def resample_u8(descs, tables, workspace):
+    """b200vton_resample_u8 on a list of ResampleDesc: tables, an int32 CUDA tensor holding every descriptor's bounds
+    and fixed-point coefficients (the descriptors' offsets index it); workspace, a uint8 CUDA tensor for the
+    intermediate rows (the descriptors' tmp_offset index it)."""
+    fn = _optional("b200vton_resample_u8")
+    if tables.dtype != torch.int32 or not tables.is_cuda or not tables.is_contiguous():
+        raise ValueError("resample_u8: tables must be a contiguous CUDA int32 tensor")
+    if workspace.dtype != torch.uint8 or not workspace.is_cuda or not workspace.is_contiguous():
+        raise ValueError("resample_u8: workspace must be a contiguous CUDA uint8 tensor")
+    arr = (ResampleDesc * len(descs))(*descs)
+    dev = _descs_to_device(arr, tables.device)
+    _check(fn(arr, _p(dev), len(descs), _p(tables), tables.numel(), _p(workspace), workspace.numel(), _stream()),
+           "b200vton_resample_u8")
+
+
+def paste_u8(descs, device):
+    """b200vton_paste_u8 on a list of PasteDesc."""
+    fn = _optional("b200vton_paste_u8")
+    arr = (PasteDesc * len(descs))(*descs)
+    dev = _descs_to_device(arr, device)
+    _check(fn(arr, _p(dev), len(descs), _stream()), "b200vton_paste_u8")

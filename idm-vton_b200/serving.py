@@ -25,11 +25,20 @@ from .denoise import GarmentKVCache
 
 @dataclasses.dataclass
 class TryOnRequest:
-    """One person x one garment. Tensors follow the keyword set of inference.py:397-414 for a batch of 1."""
+    """One person x one garment. Tensors follow the keyword set of inference.py:397-414 for a batch of 1.
+
+    A photo request passes image=None and `photo`: a full-resolution photo of any size (PIL RGB, or uint8 [H, W, 3] on
+    the CPU or the GPU) or a photo.PreparedPhoto entry (not resampled again). The server crops it to its aspect,
+    resamples it to its height x width with Pillow's filter (photo.prepare_photos) and pastes the output back into the
+    photo (photo.paste_back, `paste`: "crop" replaces the whole box, "mask" only the masked pixels). mask_image and
+    pose_img may then come at the server size, as below, or at photo size (mask: PIL "L" / "1" or uint8 / bool [H, W];
+    pose: PIL RGB or uint8 [H, W, 3]); with a PreparedPhoto that holds them they may be None. The result is at photo
+    size: a PIL image ("pil"), a uint8 [H, W, 3] CUDA tensor ("pt"), a uint8 [H, W, 3] numpy array ("np"), or the
+    final latents ("latent")."""
     garment_id: Hashable
-    image: torch.Tensor                 # [3,H,W] in [0,1]
-    mask_image: torch.Tensor            # [1,H,W]
-    pose_img: torch.Tensor              # [3,H,W] in [-1,1]
+    image: Optional[torch.Tensor]       # [3,H,W] in [0,1]; None with `photo`
+    mask_image: Any                     # [1,H,W]
+    pose_img: Any                       # [3,H,W] in [-1,1]
     prompt_embeds: torch.Tensor         # [77,2048]
     negative_prompt_embeds: torch.Tensor
     pooled_prompt_embeds: torch.Tensor  # [1280]
@@ -41,6 +50,8 @@ class TryOnRequest:
     ticket: Any = None
     seed: Optional[int] = None          # ContinuousTryOnServer: this request's generator (TryOnServer ignores it)
     sampling: Optional[Hashable] = None  # the name of the server's SamplingPreset; None: the server's default preset
+    photo: Any = None                   # a full-resolution photo or a photo.PreparedPhoto (image=None then)
+    paste: str = "crop"                 # photo requests: "crop" (the demo's paste-back) or "mask"
 
 
 @dataclasses.dataclass
@@ -105,6 +116,117 @@ def _encode_garment(pipe, src, seed, device, dtype):
                 text_embeds_cloth=src.text_embeds_cloth[None].to(device=device, dtype=dtype))
 
 
+def _check_photo_request(req, height, width):
+    """Submit-time checks of a request with `photo` (ValueError): no `image` beside it, a supported photo, a mask and a
+    pose at the server size or at the photo's, and a paste mode."""
+    if req.photo is None:
+        return
+    from . import photo as P
+    if req.image is not None:
+        raise ValueError("a request with `photo` passes image=None: the server makes the image from the photo")
+    if req.paste not in P.PASTE_MODES:
+        raise ValueError(f"paste must be one of {P.PASTE_MODES}, got {req.paste!r}")
+    P.check_photo(req.photo)
+    size = P.photo_size(req.photo)
+    prepared = req.photo if isinstance(req.photo, P.PreparedPhoto) else None
+    if prepared is not None and tuple(prepared.image.shape[-2:]) != (height, width):
+        raise ValueError(f"the photo was prepared at {tuple(prepared.image.shape[-2:])}, the server runs at "
+                         f"{(height, width)}")
+    if prepared is None:
+        P.check_crop(size, height, width)
+    for value, kind, check in ((req.mask_image, "mask", P.mask_size), (req.pose_img, "pose", P.pose_size)):
+        if value is not None:
+            check(value, size, height, width)
+        elif prepared is None or getattr(prepared, kind) is None:
+            raise ValueError(f"a photo request needs its {'mask_image' if kind == 'mask' else 'pose_img'} (at the "
+                             "server's size or the photo's), or a PreparedPhoto that holds it")
+
+
+def _prepare_photos(reqs, height, width, filter):
+    """The PreparedPhoto of each photo request of `reqs` (None for the others), one resample call for all of them:
+    photo-size masks and poses are resampled with the photo."""
+    from . import photo as P
+    idx = [i for i, r in enumerate(reqs) if r.photo is not None]
+    out = [None] * len(reqs)
+    if not idx:
+        return out
+    photo_size = lambda r, v, fn: v if v is not None and fn(v, P.photo_size(r.photo), height, width) == "photo" \
+        else None  # noqa: E731
+    entries = P.prepare_photos([reqs[i].photo for i in idx], height, width, filter=filter,
+                               masks=[photo_size(reqs[i], reqs[i].mask_image, P.mask_size) for i in idx],
+                               poses=[photo_size(reqs[i], reqs[i].pose_img, P.pose_size) for i in idx])
+    for i, e in zip(idx, entries):
+        out[i] = e
+    return out
+
+
+def _prepare_photos_or_drop(reqs, height, width, filter):
+    """(entries, failed): _prepare_photos of `reqs` in one call. If that call raises, each photo request is prepared
+    on its own, and the ones that still raise come back in `failed` ({index: exception}, no entry), so one bad request
+    cannot stop the server. A library without the photo kernels raises (NotImplementedError) for all of them."""
+    try:
+        return _prepare_photos(reqs, height, width, filter), {}
+    except NotImplementedError:
+        raise
+    except (ValueError, RuntimeError):
+        entries, failed = [None] * len(reqs), {}
+        for i, r in enumerate(reqs):
+            if r.photo is None:
+                continue
+            try:
+                entries[i] = _prepare_photos([r], height, width, filter)[0]
+            except NotImplementedError:
+                raise
+            except (ValueError, RuntimeError) as exc:
+                failed[i] = exc
+        return entries, failed
+
+
+def _person_inputs(req, entry):
+    """(image [3,H,W], mask [1,H,W], pose [3,H,W]) of a request at the server size: its own tensors, or for a photo
+    request the prepared crop, with the resampled mask / pose where they came at photo size (photo.mask_size and
+    photo.pose_size decide which size a mask or pose is, here as at submit)."""
+    if entry is None:
+        return req.image, req.mask_image, req.pose_img
+    from . import photo as P
+    h, w = entry.image.shape[-2:]
+    server = lambda v, fn: v if v is not None and fn(v, entry.size, h, w) == "server" else None  # noqa: E731
+    mask, pose = server(req.mask_image, P.mask_size), server(req.pose_img, P.pose_size)
+    return entry.image, entry.mask if mask is None else mask, entry.pose if pose is None else pose
+
+
+def _photo_result(full, output_type):
+    if output_type == "pt":
+        return full
+    a = full.cpu().numpy()
+    if output_type == "np":
+        return a
+    import PIL.Image
+    return PIL.Image.fromarray(a)
+
+
+def _decode_with_photos(pipe, output_type, latents, entries, reqs):
+    """Images of requests that finish together, from their final latents (output_type is not "latent"): one VAE decode;
+    rows without a photo get the pipeline's own post-processing of their rows (the bits they get without photos);
+    photo rows get the uint8 output the pipeline's "pil" is made of, pasted back into their photos in one launch."""
+    from . import lib as L
+    from . import photo as P
+    decoded = pipe._decode_latents(latents)
+    out = [None] * len(entries)
+    plain = [i for i, e in enumerate(entries) if e is None]
+    photo = [i for i, e in enumerate(entries) if e is not None]
+    if plain:
+        imgs = pipe._postprocess(decoded if not photo else decoded[plain], output_type)
+        for j, i in enumerate(plain):
+            out[i] = imgs[j]
+    _, u8 = L.postprocess_image(decoded if not plain else decoded[photo], want_pt=False, want_u8=True)
+    full = P.paste_back([entries[i] for i in photo], u8, [reqs[i].paste for i in photo],
+                        masks=[_person_inputs(reqs[i], entries[i])[1] for i in photo])
+    for j, i in enumerate(photo):
+        out[i] = _photo_result(full[j], output_type)
+    return out
+
+
 def _seeded_global_rng(device, seed):
     """The reference draws the pose latents' posterior sample from the GLOBAL generator (src/tryon_pipeline.py:1646
     passes no generator): with a seed, the global CPU / device generators are forked around the draw and seeded (their
@@ -126,10 +248,15 @@ class TryOnServer:
     """Batch mode: requests that wear the same garment and use the same sampling preset run as one pipeline call.
     presets: {name: SamplingPreset} (a request picks one by `sampling`; default_preset when it names none); each batch
     calls the pipeline with its preset's arguments, its scheduler (a private copy) installed for the call. None: one
-    preset from num_inference_steps and guidance_scale with the pipeline's scheduler."""
+    preset from num_inference_steps and guidance_scale with the pipeline's scheduler.
+    Photo requests (TryOnRequest.photo) whose preparation fails are dropped from their batch, which still runs; their
+    tickets map to the exception in `failed`."""
 
     def __init__(self, pipe, height=1024, width=768, num_inference_steps=30, guidance_scale=2.0, max_batch=8, seed=None,
-                 garment_cache_bytes=40 << 30, output_type="pt", presets=None, default_preset=None):
+                 garment_cache_bytes=40 << 30, output_type="pt", presets=None, default_preset=None, photo_filter="bicubic"):
+        from .photo import _check_filter
+        _check_filter(photo_filter)
+        self.photo_filter = photo_filter
         self.pipe = pipe
         self.height, self.width = height, width
         self.num_inference_steps, self.guidance_scale = num_inference_steps, guidance_scale
@@ -146,12 +273,14 @@ class TryOnServer:
         self.garments = {}                          # garment_id -> dict(latents, ip_adapter_image, text_embeds_cloth)
         self._next_ticket = 0
         self.stats = collections.Counter()
+        self.failed = {}                             # ticket -> exception: photo requests whose preparation failed
         if garment_cache_bytes:
             pipe.garment_cache = GarmentKVCache(garment_cache_bytes)
 
     # ---------------------------------------------------------------------------------------------
     def submit(self, req: TryOnRequest):
         name = _preset_name(self, req)
+        _check_photo_request(req, self.height, self.width)
         if req.garment_id not in self.garments and all(g != req.garment_id for g, _ in self.queue) and \
                 (req.cloth is None or req.ip_adapter_image is None or req.text_embeds_cloth is None):
             raise ValueError(f"garment {req.garment_id!r} is new: cloth, ip_adapter_image and text_embeds_cloth are required")
@@ -197,6 +326,26 @@ class TryOnServer:
         gen = torch.Generator(device).manual_seed(self.seed) if self.seed is not None else None
         g = self._garment(gid, batch, device, dtype)
         stack = lambda name, dt=None: torch.stack([getattr(r, name) for r in batch]).to(device=device, dtype=dt)  # noqa: E731
+        entries, failed = _prepare_photos_or_drop(batch, self.height, self.width, self.photo_filter)
+        if failed:            # dropped from the batch; the rest of it runs
+            for i, exc in failed.items():
+                self.failed[batch[i].ticket] = exc
+            self.stats["failed"] += len(failed)
+            batch = [r for i, r in enumerate(batch) if i not in failed]
+            entries = [e for i, e in enumerate(entries) if i not in failed]
+            if not batch:
+                return {}
+        photos = any(e is not None for e in entries)
+        if photos:            # the photo requests' crops (one resample launch) beside the others' tensors
+            person = [_person_inputs(r, e) for r, e in zip(batch, entries)]
+            person = {k: torch.stack([p[j].to(device=device) for p in person]) for j, k in enumerate(("image",
+                                                                                                      "mask_image",
+                                                                                                      "pose_img"))}
+            person["pose_img"] = person["pose_img"].to(dtype)
+        else:
+            person = dict(image=stack("image"), mask_image=stack("mask_image"), pose_img=stack("pose_img", dtype))
+        # photo rows are decoded here, after the call, so that they can be pasted back (output_type "latent" skips it)
+        out_type = "latent" if photos else self.output_type
         # eta and guidance_rescale are passed only when a preset sets them (the pipeline's defaults otherwise)
         extra = {k: getattr(preset, k) for k in ("eta", "guidance_rescale") if getattr(preset, k)}
         # the pose latents' sample comes from the global generator: seeded around the call (_seeded_global_rng), so a
@@ -206,10 +355,16 @@ class TryOnServer:
                           pooled_prompt_embeds=stack("pooled_prompt_embeds", dtype),
                           negative_pooled_prompt_embeds=stack("negative_pooled_prompt_embeds", dtype),
                           num_inference_steps=preset.num_inference_steps, generator=gen, strength=preset.strength,
-                          pose_img=stack("pose_img", dtype), text_embeds_cloth=g["text_embeds_cloth"], cloth=g["latents"],
-                          mask_image=stack("mask_image"), image=stack("image"), height=self.height, width=self.width,
-                          ip_adapter_image=g["ip_adapter_image"], guidance_scale=preset.guidance_scale,
-                          output_type=self.output_type, garment_keys=[gid], **extra)[0]
+                          pose_img=person["pose_img"], text_embeds_cloth=g["text_embeds_cloth"], cloth=g["latents"],
+                          mask_image=person["mask_image"], image=person["image"], height=self.height,
+                          width=self.width, ip_adapter_image=g["ip_adapter_image"],
+                          guidance_scale=preset.guidance_scale, output_type=out_type, garment_keys=[gid], **extra)[0]
+        if photos:
+            latents = pipe._last_latents
+            if self.output_type == "latent":
+                images = [latents[i] if e is not None else images[i] for i, e in enumerate(entries)]
+            else:
+                images = _decode_with_photos(pipe, self.output_type, latents, entries, batch)
         self.stats["batches"] += 1
         self.stats["images"] += len(batch)
         return {r.ticket: images[i] for i, r in enumerate(batch)}
@@ -265,10 +420,16 @@ class ContinuousTryOnServer:
     than DDPM (NotImplementedError); presets with guidance_scale <= 1 beside presets with CFG (ValueError); schedulers
     other than DDPM / DDIM / Euler / DPM-Solver++; a library without the per-slot step kernels, the mixed-kind step
     kernel (b200vton_cfg_step_mixed_rows) when presets need it, or, in pool mode, b200vton_attention_rows
-    (NotImplementedError naming the symbol). An unknown preset name is refused at submit (ValueError)."""
+    (NotImplementedError naming the symbol). An unknown preset name is refused at submit (ValueError).
+    Photo requests (TryOnRequest.photo) are prepared at admission; one whose preparation fails is dropped from the queue
+    without taking a slot, and its ticket maps to the exception in `failed`."""
 
     def __init__(self, pipe, height=1024, width=768, slots=4, num_inference_steps=30, guidance_scale=2.0, seed=None,
-                 output_type="pt", eta=0.0, garment_kv_bytes=None, presets=None, default_preset=None):
+                 output_type="pt", eta=0.0, garment_kv_bytes=None, presets=None, default_preset=None,
+                 photo_filter="bicubic"):
+        from .photo import _check_filter
+        _check_filter(photo_filter)
+        self.photo_filter = photo_filter
         self.pipe = pipe
         self.height, self.width = height, width
         self.S = int(slots)
@@ -296,10 +457,12 @@ class ContinuousTryOnServer:
         self.last_latents = {}                       # ticket -> final latents of the requests the last step() finished
         self._next_ticket = 0
         self.stats = collections.Counter()
+        self.failed = {}                             # ticket -> exception: photo requests whose preparation failed
 
     # ---------------------------------------------------------------------------------------------
     def submit(self, req: TryOnRequest):
         _preset_name(self, req)
+        _check_photo_request(req, self.height, self.width)
         known = req.garment_id in self.garments or any(r.garment_id == req.garment_id for r in self.waiting) or any(
             e is not None and e["req"].garment_id == req.garment_id for e in self.slots)
         if not known:
@@ -434,16 +597,17 @@ class ContinuousTryOnServer:
             self.stats["garments_encoded"] += 1
         return g
 
-    def _prepare_request(self, req, gen):
+    def _prepare_request(self, req, gen, entry=None):
         """The pipeline's own preparation of one person (batch 1, the request's preset and its scheduler installed):
         pre-processing, initial latents (with strength < 1 the image's VAE sample, then the noise, added to it at the
         first timestep), mask and masked-image latents, pose latents, prompt and added-condition embeddings — drawing
-        from `gen` in the pipeline's order. Returns the keyword arguments of SlotDenoiser.admit except the garment's."""
+        from `gen` in the pipeline's order. entry: the request's PreparedPhoto (photo requests). Returns the keyword
+        arguments of SlotDenoiser.admit except the garment's."""
         name = _preset_name(self, req)
         with _scheduler_installed(self.pipe, self._schedulers[name]):
-            return self._prepare_with(req, gen, self._preset(name).strength, self._timesteps[name])
+            return self._prepare_with(req, gen, self._preset(name).strength, self._timesteps[name], entry)
 
-    def _prepare_with(self, req, gen, strength, timesteps):
+    def _prepare_with(self, req, gen, strength, timesteps, entry=None):
         pipe = self.pipe
         device, dtype = pipe._execution_device, pipe.unet.dtype
         do_cfg = pipe.do_classifier_free_guidance
@@ -454,15 +618,16 @@ class ContinuousTryOnServer:
             negative_prompt_embeds=req.negative_prompt_embeds[None].to(device=device, dtype=dtype),
             pooled_prompt_embeds=req.pooled_prompt_embeds[None].to(device=device, dtype=dtype),
             negative_pooled_prompt_embeds=req.negative_pooled_prompt_embeds[None].to(device=device, dtype=dtype))
+        image, mask_image, pose_img = _person_inputs(req, entry)
         init_image, mask, masked_image, mask_latent = pipe._preprocess_image_mask(
-            req.image[None].to(device=device), req.mask_image[None].to(device=device), None, H, W)
+            image[None].to(device=device), mask_image[None].to(device=device), None, H, W)
         latents, = pipe.prepare_latents(1, pipe.vae.config.latent_channels, H, W, pe.dtype, device, gen, None,
                                         image=init_image, timestep=timesteps[:1],
                                         is_strength_max=strength == 1.0)                                     # draw 1
         mask, masked_lat = pipe.prepare_mask_latents(mask, masked_image, 1, H, W, pe.dtype, device, gen, do_cfg,
                                                      _mask_latent=mask_latent)                               # draw 2
         with _seeded_global_rng(device, self._seed(req)):
-            pose = pipe._pose_latents(req.pose_img[None].to(device=device, dtype=pe.dtype), pe.dtype)        # global
+            pose = pipe._pose_latents(pose_img[None].to(device=device, dtype=pe.dtype), pe.dtype)            # global
         proj_dim = int(ppe.shape[-1]) if pipe.text_encoder_2 is None else pipe.text_encoder_2.config.projection_dim
         size = (latents.shape[-2] * pipe.vae_scale_factor, latents.shape[-1] * pipe.vae_scale_factor)
         add_time_ids, add_neg_time_ids = pipe._get_add_time_ids(size, (0, 0), size, 6.0, 2.5, size, (0, 0), size,
@@ -493,25 +658,34 @@ class ContinuousTryOnServer:
             self._configure()
             self._kv_format = fmt
         device, dtype = self.pipe._execution_device, self.pipe.unet.dtype
-        for s in free:
-            if not self.waiting:
-                break
-            req = self.waiting.popleft()
-            g = self._garment(req, device, dtype)
-            seed = self._seed(req)
-            gen = torch.Generator(device).manual_seed(seed) if seed is not None else None
-            prep = self._prepare_request(req, gen)
-            if self.mixed:             # the slot runs plan j; the garment's page is keyed by that plan's timesteps
-                j = self._plan_index[_preset_name(self, req)]
-                T, t_table = self.plans[j].T, self.plans[j].t_table[:self.plans[j].T]
-                key = (req.garment_id, tuple(float(t) for t in t_table))
-            else:
-                j, T, t_table, key = None, self.T, None, req.garment_id
-            page = None if self.garment_kv_bytes is None else self._pin_page(key, g, t_table)
-            self.den.admit(s, cloth_latents=g["latents"], image_embeds=g["image_embeds"],
-                           text_embeds_cloth=g["text_embeds_cloth"], page=page, **prep)
-            self.slots[s] = dict(req=req, gen=gen, step=0, page=page, plan=j, T=T)
-            self.stats["admitted"] += 1
+        while free and self.waiting:       # again when a dropped request left a slot free
+            n = min(len(free), len(self.waiting))
+            heads = [self.waiting[i] for i in range(n)]
+            entries, failed = _prepare_photos_or_drop(heads, self.height, self.width, self.photo_filter)
+            slots = iter(free)
+            for i, entry in enumerate(entries):
+                req = self.waiting.popleft()
+                g = self._garment(req, device, dtype)       # a dropped request's garment stays known to later requests
+                if i in failed:
+                    self.failed[req.ticket] = failed[i]
+                    self.stats["failed"] += 1
+                    continue
+                s = next(slots)
+                seed = self._seed(req)
+                gen = torch.Generator(device).manual_seed(seed) if seed is not None else None
+                prep = self._prepare_request(req, gen) if entry is None else self._prepare_request(req, gen, entry)
+                if self.mixed:             # the slot runs plan j; the garment's page is keyed by that plan's timesteps
+                    j = self._plan_index[_preset_name(self, req)]
+                    T, t_table = self.plans[j].T, self.plans[j].t_table[:self.plans[j].T]
+                    key = (req.garment_id, tuple(float(t) for t in t_table))
+                else:
+                    j, T, t_table, key = None, self.T, None, req.garment_id
+                page = None if self.garment_kv_bytes is None else self._pin_page(key, g, t_table)
+                self.den.admit(s, cloth_latents=g["latents"], image_embeds=g["image_embeds"],
+                               text_embeds_cloth=g["text_embeds_cloth"], page=page, **prep)
+                self.slots[s] = dict(req=req, gen=gen, step=0, page=page, plan=j, T=T, photo=entry)
+                self.stats["admitted"] += 1
+            free = [s for s, e in enumerate(self.slots) if e is None]
 
     def _pin_page(self, key, g, t_table=None):
         """Pool mode: the page holding `key` (the garment id; with the mixed-kind step, (garment id, the plan's
@@ -571,7 +745,13 @@ class ContinuousTryOnServer:
         final = latents[done].clone()
         tickets = [self.slots[s]["req"].ticket for s in done]
         self.last_latents = dict(zip(tickets, final))
-        images = self._decode(final)
+        entries = [self.slots[s]["photo"] for s in done]
+        if self.output_type != "latent" and any(e is not None for e in entries):
+            # photo requests finishing at this step are pasted back in one launch
+            images = _decode_with_photos(self.pipe, self.output_type, final, entries,
+                                         [self.slots[s]["req"] for s in done])
+        else:
+            images = self._decode(final)
         for s in done:
             den.release(s)
             if self.slots[s]["page"] is not None:      # the page stays resident as a cache entry

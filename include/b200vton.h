@@ -318,6 +318,58 @@ int b200vton_preprocess_inpaint(const void* image, const void* mask, int mask_ch
  * (out_pt, may be NULL) and/or uint8 NHWC round(255 y) (out_u8, may be NULL; what "np"/"pil" produce, 4x less D2H). */
 int b200vton_postprocess_image(const void* x, int nhwc, int B, int H, int W, void* out_pt, void* out_u8, void* stream);
 
+/* Full-resolution photos (INTEGRATION.md, "Full-resolution photos"; the reference demo's auto-crop, resize and
+ * paste-back, gradio_demo/app.py:135-147, 236-239). Both entry points are integer-only and deterministic.
+ *
+ * b200vton_resample_u8: Pillow's Image.resize with a convolution filter (ImagingResample, 8 bits per channel) of a
+ * batch of uint8 HWC crops (channels 1 or 3), each with its own sizes. The crop [crop_x, crop_x + crop_w) x
+ * [crop_y, crop_y + crop_h) of `src` is the image: taps are clipped to the crop, never to the photo around it.
+ * Per axis, `tables` holds at bounds_* two int32 per output (first tap, tap count) and at coefs_* ksize_* int32 per
+ * output: Pillow's coefficients (precompute_coeffs) in 22-bit fixed point (normalize_coeffs_8bpc). need_x / need_y
+ * say whether Pillow runs that pass (output size != crop size on that axis). The horizontal pass runs first:
+ *   tmp[r][x] = clip8(2^21 + sum_k src[tmp_first + r][first_x + k] * coef_x[k]),   r < tmp_rows,
+ * into `workspace` at tmp_offset (tmp_rows x out_w x channels bytes; tmp_first..tmp_first + tmp_rows are the crop rows
+ * the vertical pass reads), then the vertical pass on tmp (or on the crop when need_x == 0):
+ *   dst[y][x] = clip8(2^21 + sum_k tmp[first_y - tmp_first + k][x] * coef_y[k]),   clip8(s) = clamp(s >> 22, 0, 255).
+ * With neither pass the crop is copied. out_f32 (may be NULL) receives the result as fp32 NCHW [channels, out_h, out_w]:
+ * f32_mode 0 = v / 255 (np.asarray(img, np.float32) / 255), 1 = (v / 255 - 0.5) / 0.5 (ToTensor + Normalize(0.5, 0.5)).
+ * descs (host) is checked and sizes the grid; descs_dev is the same table in device memory, read by the kernels. The
+ * table contents (first taps and counts within the crop, as Pillow's bounds are) are not checked. Two launches (one per
+ * pass), each covering the whole batch. n <= 4096. */
+typedef struct b200vton_resample_desc {
+  const uint8_t* src;
+  int64_t src_pitch;  /* bytes per row */
+  int32_t src_w, src_h, crop_x, crop_y, crop_w, crop_h;
+  uint8_t* dst;
+  int64_t dst_pitch;
+  float* out_f32;
+  int32_t out_w, out_h, channels, f32_mode;
+  int32_t bounds_x, coefs_x, ksize_x, need_x;
+  int32_t bounds_y, coefs_y, ksize_y, need_y;
+  int64_t tmp_offset;
+  int32_t tmp_first, tmp_rows;
+} b200vton_resample_desc;
+int b200vton_resample_u8(const b200vton_resample_desc* descs, const void* descs_dev, int n, const int32_t* tables,
+                         int64_t table_len, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* b200vton_paste_u8: the full-resolution results of a batch of photos (uint8 HWC, 3 channels) in one launch:
+ * dst = photo outside the box [box_x, box_x + box_w) x [box_y, box_y + box_h); inside it image[y - box_y][x - box_x]
+ * (the resampled output, box_w x box_h x 3), or, with a mask (1 channel, mask_w x mask_h at (mask_x, mask_y) in photo
+ * coordinates, covering the box), image where mask >= 128 and photo elsewhere. dst may not alias photo or image. */
+typedef struct b200vton_paste_desc {
+  const uint8_t* photo;
+  int64_t photo_pitch;
+  uint8_t* dst;
+  int64_t dst_pitch;
+  const uint8_t* image;
+  int64_t image_pitch;
+  const uint8_t* mask;
+  int64_t mask_pitch;
+  int32_t width, height, box_x, box_y, box_w, box_h;
+  int32_t mask_x, mask_y, mask_w, mask_h;
+} b200vton_paste_desc;
+int b200vton_paste_u8(const b200vton_paste_desc* descs, const void* descs_dev, int n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
