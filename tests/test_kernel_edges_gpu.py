@@ -658,13 +658,28 @@ def test_references_match_torch_float64():
     assert torch.allclose(gelu64(xl), F.gelu(xl), atol=1e-14) and torch.allclose(quick_gelu64(xl), xl * torch.sigmoid(1.702 * xl))
 
 
-def test_gemm_operands_on_the_grid_accumulate_exactly():
-    """The premise of the bit-exact epilogue / convolution cases: grid operands' products and sums are exact in fp32."""
-    a = grid16(300, 1152, scale=1.0, seed=11)
-    w = grid16(64, 1152, scale=0.25, seed=12)
+def grid_sums_exact(K):
+    """Grid operands (a: scale 1, w: scale 1/4) accumulate exactly in fp32 at depth K: every product is a multiple of
+    2^-8 of magnitude <= 1/4, so every partial sum, in any order, is a multiple of 2^-8 below K / 4, exact while
+    K / 4 < 2^16 (fewer than 2^24 steps of 2^-8). One row reaches the largest sum the grid allows."""
+    a = grid16(300, K, scale=1.0, seed=11)
+    w = grid16(64, K, scale=0.25, seed=12)
+    a[0], w[0] = 1.0, 0.25
     acc64 = a.double() @ w.double().t()
     assert torch.equal(acc64.float().double(), acc64)
-    assert acc64.abs().max().item() < 2 ** 14              # partial sums are multiples of 2^-8: < 2^22 steps, exact
+    assert acc64.abs().max().item() == K / 4 < 2 ** 16
+    assert torch.equal((acc64 * 256).round(), acc64 * 256)
+
+
+def test_gemm_operands_on_the_grid_accumulate_exactly():
+    """The premise of the bit-exact epilogue / convolution cases: grid operands' products and sums are exact in fp32."""
+    grid_sums_exact(1152)
+
+
+def test_grid_operands_exact_at_the_largest_full_size_k():
+    """The same premise at 9 * 2560, the largest K a full-size step launches (conv1 of the first up-block resnets, after
+    the 1280 + 1280 skip concat; tests/test_launch_inventory_gpu.py checks its inventory against it)."""
+    grid_sums_exact(9 * 2560)
 
 
 @pytest.mark.parametrize("name,M,N,K,rps,act,mutants", EPI_CASES, ids=[c[0] for c in EPI_CASES])
