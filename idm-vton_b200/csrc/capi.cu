@@ -82,6 +82,8 @@ int cfg_mixed_rows_impl(const void* eps, int ldc, int B, int C, int H, int W, co
 int resample_u8_impl(const b200vton_resample_desc* descs, const void* descs_dev, int n, const int32_t* tables,
                      long long table_len, void* workspace, long long workspace_bytes, cudaStream_t stream);
 int paste_u8_impl(const b200vton_paste_desc* descs, const void* descs_dev, int n, cudaStream_t stream);
+int clip_pixels_u8_impl(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table, float* out,
+                        cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
@@ -310,6 +312,10 @@ int b200vton_resample_u8(const b200vton_resample_desc* descs, const void* descs_
 }
 int b200vton_paste_u8(const b200vton_paste_desc* descs, const void* descs_dev, int n, void* stream) {
   return vton::paste_u8_impl(descs, descs_dev, n, S(stream));
+}
+int b200vton_clip_pixels_u8(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table,
+                            float* out, void* stream) {
+  return vton::clip_pixels_u8_impl(descs, descs_dev, n, table, out, S(stream));
 }
 
 }  // extern "C"

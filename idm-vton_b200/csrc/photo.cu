@@ -1,7 +1,8 @@
 // Full-resolution photos (include/b200vton.h, b200vton_resample_u8 / b200vton_paste_u8): Pillow-exact resampling of
 // uint8 crops (ImagingResample's 8-bit path: fixed-point coefficients, horizontal pass into a uint8 intermediate, then
 // the vertical pass) and the paste of the resampled output back into the photo. Integer arithmetic only, so every
-// result is Pillow's to the byte and independent of the launch configuration.
+// result is Pillow's to the byte and independent of the launch configuration. b200vton_clip_pixels_u8 turns garment
+// images already resampled to the CLIP size into the image encoder's pixels through a 3 x 256 lookup table.
 //
 // A batch of photos of different sizes runs as one launch per pass: blockIdx.y selects the descriptor, and the CTAs of
 // a row stride over that image's outputs. One thread per output byte: neighbouring threads read neighbouring source
@@ -124,6 +125,24 @@ __global__ void __launch_bounds__(kThreads) paste_kernel(const b200vton_paste_de
   }
 }
 
+// CLIPImageProcessor's centre crop, rescale and normalize of a batch of CLIP-size images: out[j][c][y][x] =
+// table[c][src_j[crop_y + y][crop_x + x][c]]. One thread per output float, in NCHW order, so the stores coalesce.
+__global__ void __launch_bounds__(kThreads) clip_pixels_kernel(const b200vton_clip_desc* descs, const float* table,
+                                                               float* out) {
+  __shared__ float lut[3 * 256];
+  for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i] = table[i];
+  __syncthreads();
+  const b200vton_clip_desc d = descs[blockIdx.y];
+  constexpr int kPlane = B200VTON_CLIP_SIZE * B200VTON_CLIP_SIZE;
+  float* o = out + static_cast<long long>(blockIdx.y) * 3 * kPlane;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * kPlane; i += gridDim.x * blockDim.x) {
+    const int c = i / kPlane, rem = i - c * kPlane;
+    const int y = rem / B200VTON_CLIP_SIZE, x = rem - y * B200VTON_CLIP_SIZE;
+    const uint8_t v = d.src[static_cast<long long>(d.crop_y + y) * d.src_pitch + 3LL * (d.crop_x + x) + c];
+    o[i] = lut[c * 256 + v];
+  }
+}
+
 unsigned grid_x(long long max_total) {
   const long long want = (max_total + kThreads - 1) / kThreads;
   const long long cap = 8LL * num_sms();
@@ -214,6 +233,29 @@ int paste_u8_impl(const b200vton_paste_desc* descs, const void* descs_dev, int n
     max_total = std::max(max_total, 3LL * d.width * d.height);
   }
   paste_kernel<<<dim3(grid_x(max_total), n), kThreads, 0, stream>>>(static_cast<const b200vton_paste_desc*>(descs_dev));
+  count_launch();
+  VTON_CUDA(cudaGetLastError());
+  return kOk;
+}
+
+int clip_pixels_u8_impl(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table, float* out,
+                        cudaStream_t stream) {
+  VTON_CHECK_ARG(descs && descs_dev && n > 0 && n <= kMaxDescs,
+                 "clip_pixels_u8: need 1..%d descriptors (host and device)", kMaxDescs);
+  VTON_CHECK_ARG(aligned_to(descs_dev, 8), "clip_pixels_u8: descs_dev must be 8-byte aligned");
+  VTON_CHECK_ARG(table && out && aligned_to(table, 4) && aligned_to(out, 4),
+                 "clip_pixels_u8: table and out must be non-null and 4-byte aligned");
+  constexpr int S = B200VTON_CLIP_SIZE;
+  for (int j = 0; j < n; ++j) {
+    const b200vton_clip_desc& d = descs[j];
+    VTON_CHECK_ARG(d.src && d.src_w > 0 && d.src_h > 0 && d.src_pitch >= 3LL * d.src_w,
+                   "clip_pixels_u8: descriptor %d: null src, empty image or pitch below a row", j);
+    VTON_CHECK_ARG(d.crop_x >= 0 && d.crop_y >= 0 && d.crop_x + S <= d.src_w && d.crop_y + S <= d.src_h,
+                   "clip_pixels_u8: descriptor %d: crop (%d,%d) %dx%d outside the %dx%d image", j, d.crop_x, d.crop_y,
+                   S, S, d.src_w, d.src_h);
+  }
+  clip_pixels_kernel<<<dim3(grid_x(3LL * S * S), n), kThreads, 0, stream>>>(
+      static_cast<const b200vton_clip_desc*>(descs_dev), table, out);
   count_launch();
   VTON_CUDA(cudaGetLastError());
   return kOk;

@@ -50,7 +50,7 @@ SIGNATURES = {
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
 # step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears,
 # the per-sample-row attention of its pool mode, the FP8 garment K/V (quantizer and attention) and the full-resolution
-# photo kernels (resampler and paste-back).
+# photo kernels (resampler, paste-back and the garment's CLIP pixels).
 # `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
@@ -66,6 +66,7 @@ OPTIONAL_SIGNATURES = {
                                _i, _i, _vp, _vp, _f, _i, _vp],
     "b200vton_resample_u8": [_vp, _vp, _i, _vp, _i64, _vp, _i64, _vp],
     "b200vton_paste_u8": [_vp, _vp, _i, _vp],
+    "b200vton_clip_pixels_u8": [_vp, _vp, _i, _vp, _vp, _vp],
 }
 _present = set()
 
@@ -924,3 +925,27 @@ def paste_u8(descs, device):
     arr = (PasteDesc * len(descs))(*descs)
     dev = _descs_to_device(arr, device)
     _check(fn(arr, _p(dev), len(descs), _stream()), "b200vton_paste_u8")
+
+
+CLIP_SIZE = 224        # B200VTON_CLIP_SIZE
+
+
+class ClipDesc(ctypes.Structure):
+    """b200vton_clip_desc (include/b200vton.h): one CLIP-size image and the origin of its 224 x 224 crop."""
+    _fields_ = [("src", _vp), ("src_pitch", _i64), ("src_w", _c.c_int32), ("src_h", _c.c_int32),
+                ("crop_x", _c.c_int32), ("crop_y", _c.c_int32)]
+
+
+def clip_pixels_u8(descs, table, out):
+    """b200vton_clip_pixels_u8 on a list of ClipDesc: table, a contiguous fp32 CUDA tensor of 3 x 256 entries; out, a
+    contiguous fp32 CUDA tensor [len(descs), 3, 224, 224]."""
+    fn = _optional("b200vton_clip_pixels_u8")
+    if table.dtype != torch.float32 or not table.is_cuda or not table.is_contiguous() or table.numel() != 3 * 256:
+        raise ValueError("clip_pixels_u8: table must be a contiguous CUDA fp32 tensor of 3 x 256 entries")
+    if out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or \
+            tuple(out.shape) != (len(descs), 3, CLIP_SIZE, CLIP_SIZE):
+        raise ValueError(f"clip_pixels_u8: out must be a contiguous CUDA fp32 tensor [{len(descs)}, 3, {CLIP_SIZE}, "
+                         f"{CLIP_SIZE}], got {out.dtype} {tuple(out.shape)} on {out.device}")
+    arr = (ClipDesc * len(descs))(*descs)
+    dev = _descs_to_device(arr, out.device)
+    _check(fn(arr, _p(dev), len(descs), _p(table), _p(out), _stream()), "b200vton_clip_pixels_u8")

@@ -17,6 +17,10 @@ Steps 2 and 4 run b200vton_resample_u8, Pillow's ImagingResample restated in int
 Around a plain pipeline call:  p = prepare_photos([photo], 1024, 768);  pipe(image=p.images, ...,
 output_type="pil") ... then paste_back(p, uint8 [B, 1024, 768, 3] of the outputs). The try-on servers do both steps for
 requests that carry `photo` (serving.TryOnRequest).
+
+Garment photos (prepare_garments) follow the demo's garm_img: the whole photo resized to the server size (BICUBIC), its
+ToTensor + Normalize as `cloth`, and CLIPImageProcessor's Pillow path on it as the IP-Adapter's pixels (the CLIP resize
+by b200vton_resample_u8, the centre crop and the 3 x 256 rescale / normalize table by b200vton_clip_pixels_u8).
 """
 import dataclasses
 import functools
@@ -393,6 +397,95 @@ def prepare_photos(photos, height, width, filter="bicubic", masks=None, poses=No
 def _crop_rect(e):
     x0, y0, x1, y1 = e.crop
     return x0, y0, x1 - x0, y1 - y0
+
+
+# ------------------------------------------------------------------------------------------------
+# garment photos: the demo's garm_img (gradio_demo/app.py:132, 215, 232)
+# ------------------------------------------------------------------------------------------------
+CLIP_SIZE = L.CLIP_SIZE
+CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)     # CLIPImageProcessor's defaults (OpenAI CLIP)
+CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+
+
+def clip_table():
+    """float32 [3, 256]: CLIPImageProcessor's rescale and normalize of every uint8 value, as transformers computes it:
+    x = float32(float64(v) * (1 / 255)), then (x - mean) / std in float32 with the float32 mean and std."""
+    x = (np.arange(256, dtype=np.float64) * (1 / 255)).astype(np.float32)
+    mean, std = np.array(CLIP_MEAN, np.float32), np.array(CLIP_STD, np.float32)
+    return (x[None, :] - mean[:, None]) / std[:, None]
+
+
+@functools.lru_cache(maxsize=8)
+def _clip_table_on(device):
+    return torch.from_numpy(clip_table()).to(device)
+
+
+def clip_resize(width, height):
+    """CLIPImageProcessor's geometry for a width x height image: (new_w, new_h, left, top). The short side becomes 224
+    and the long side int(224 * long / short) (transformers' shortest-edge rule); the 224 x 224 centre crop starts at
+    left = (new_w - 224) // 2, top = (new_h - 224) // 2."""
+    short, long = min(width, height), max(width, height)
+    new_long = int(CLIP_SIZE * long / short)
+    new_w, new_h = (CLIP_SIZE, new_long) if width <= height else (new_long, CLIP_SIZE)
+    return new_w, new_h, (new_w - CLIP_SIZE) // 2, (new_h - CLIP_SIZE) // 2
+
+
+def check_garment(garment):
+    """ValueError unless `garment` is a PIL image of any mode (converted with .convert("RGB"), as the demo does) or a
+    uint8 [H, W, 3] tensor, with at least one pixel."""
+    if _is_pil(garment):
+        size = garment.size
+    elif torch.is_tensor(garment) and garment.dtype == torch.uint8 and garment.dim() == 3 and garment.shape[2] == 3:
+        size = (int(garment.shape[1]), int(garment.shape[0]))
+    else:
+        raise ValueError("garment_photo must be a PIL image or a uint8 [H, W, 3] tensor, got "
+                         f"{type(garment).__name__} {getattr(garment, 'dtype', '')} {tuple(getattr(garment, 'shape', ()))}")
+    if size[0] < 1 or size[1] < 1:
+        raise ValueError(f"garment_photo is empty ({size[0]}x{size[1]})")
+
+
+@dataclasses.dataclass
+class PreparedGarment:
+    """One garment at the server size, as the demo prepares garm_img:
+      image_u8: uint8 [height, width, 3] CUDA, Pillow's garm_img.convert("RGB").resize((width, height)) (BICUBIC);
+      cloth: fp32 [3, height, width] CUDA, ToTensor + Normalize([0.5], [0.5]) of it (the pipeline's `cloth`);
+      clip_pixels: fp32 [3, 224, 224] CUDA, CLIPImageProcessor()(image).pixel_values with transformers' Pillow path
+      (the pipeline's `ip_adapter_image`)."""
+    image_u8: torch.Tensor
+    cloth: torch.Tensor
+    clip_pixels: torch.Tensor
+
+
+def prepare_garments(garments, height, width):
+    """Garment photos -> PreparedGarment entries at the server size height x width, in three calls for the whole list:
+    one b200vton_resample_u8 call to the server size (writing `cloth` as it goes), one from there to the CLIP size
+    (Pillow's CLIP resize starts from the resized image, not from the photo) and one b200vton_clip_pixels_u8 launch.
+
+    garments: PIL images of any mode (converted to RGB on the host) or uint8 [H, W, 3] tensors on the CPU (staged
+    through pinned memory) or the GPU. Every input is checked before anything is uploaded or launched. For a plain
+    pipeline call: pipe(cloth=g.cloth[None].half(), ip_adapter_image=g.clip_pixels[None], ...)."""
+    garments = list(garments)
+    for g in garments:
+        check_garment(g)
+    if height < 1 or width < 1:
+        raise ValueError(f"prepare_garments: empty server size {width}x{height}")
+    if not garments:
+        return []
+    device = torch.device("cuda", torch.cuda.current_device())
+    srcs = [(_pil_u8(g if g.mode == "RGB" else g.convert("RGB"), device) if _is_pil(g) else _upload(g, device))
+            for g in garments]
+    n = len(srcs)
+    image_u8 = torch.empty((n, height, width, 3), dtype=torch.uint8, device=device)
+    cloth = torch.empty((n, 3, height, width), dtype=torch.float32, device=device)
+    _resample([(s, (0, 0, s.shape[1], s.shape[0]), image_u8[i], cloth[i], 1, "bicubic") for i, s in enumerate(srcs)],
+              device)
+    cw, ch, left, top = clip_resize(width, height)
+    small = torch.empty((n, ch, cw, 3), dtype=torch.uint8, device=device)
+    _resample([(image_u8[i], (0, 0, width, height), small[i], None, 0, "bicubic") for i in range(n)], device)
+    pixels = torch.empty((n, 3, CLIP_SIZE, CLIP_SIZE), dtype=torch.float32, device=device)
+    L.clip_pixels_u8([L.ClipDesc(src=small[i].data_ptr(), src_pitch=3 * cw, src_w=cw, src_h=ch, crop_x=left,
+                                 crop_y=top) for i in range(n)], _clip_table_on(device), pixels)
+    return [PreparedGarment(image_u8=image_u8[i], cloth=cloth[i], clip_pixels=pixels[i]) for i in range(n)]
 
 
 def paste_back(prepared, images_u8, mode="crop", masks=None):

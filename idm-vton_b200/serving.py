@@ -34,15 +34,22 @@ class TryOnRequest:
     pose_img may then come at the server size, as below, or at photo size (mask: PIL "L" / "1" or uint8 / bool [H, W];
     pose: PIL RGB or uint8 [H, W, 3]); with a PreparedPhoto that holds them they may be None. The result is at photo
     size: a PIL image ("pil"), a uint8 [H, W, 3] CUDA tensor ("pt"), a uint8 [H, W, 3] numpy array ("np"), or the
-    final latents ("latent")."""
+    final latents ("latent").
+
+    Garment side, needed the first time a garment_id is seen and ignored afterwards: its image as `cloth` and
+    `ip_adapter_image`, or as `garment_photo` (a PIL image of any mode or a uint8 [H, W, 3] tensor, any size, on the CPU
+    or the GPU; the server resizes it and makes both tensors as the demo does: photo.prepare_garments); its text as
+    `text_embeds_cloth`, or as `garment_description` (encoded once per garment with the demo's prompts: PERSON_PROMPT,
+    GARMENT_PROMPT, NEGATIVE_PROMPT). A request without the four prompt embeddings uses the person prompt of its
+    garment's description."""
     garment_id: Hashable
     image: Optional[torch.Tensor]       # [3,H,W] in [0,1]; None with `photo`
     mask_image: Any                     # [1,H,W]
     pose_img: Any                       # [3,H,W] in [-1,1]
-    prompt_embeds: torch.Tensor         # [77,2048]
-    negative_prompt_embeds: torch.Tensor
-    pooled_prompt_embeds: torch.Tensor  # [1280]
-    negative_pooled_prompt_embeds: torch.Tensor
+    prompt_embeds: Optional[torch.Tensor] = None         # [77,2048]; the four: all given or all None
+    negative_prompt_embeds: Optional[torch.Tensor] = None
+    pooled_prompt_embeds: Optional[torch.Tensor] = None  # [1280]
+    negative_pooled_prompt_embeds: Optional[torch.Tensor] = None
     # garment side (needed the first time a garment_id is seen; ignored afterwards)
     cloth: Optional[torch.Tensor] = None             # [3,H,W] in [-1,1]
     ip_adapter_image: Optional[torch.Tensor] = None  # [3,224,224] CLIP-preprocessed garment image
@@ -52,6 +59,109 @@ class TryOnRequest:
     sampling: Optional[Hashable] = None  # the name of the server's SamplingPreset; None: the server's default preset
     photo: Any = None                   # a full-resolution photo or a photo.PreparedPhoto (image=None then)
     paste: str = "crop"                 # photo requests: "crop" (the demo's paste-back) or "mask"
+    garment_photo: Any = None           # instead of cloth and ip_adapter_image
+    garment_description: Optional[str] = None  # instead of text_embeds_cloth (and of the prompt embeddings)
+
+
+# The demo's prompts (gradio_demo/app.py:178-179, 193-194) for a garment description d: the person prompt
+# PERSON_PROMPT + d with classifier-free guidance against NEGATIVE_PROMPT, the garment prompt GARMENT_PROMPT + d without.
+PERSON_PROMPT = "model is wearing "
+GARMENT_PROMPT = "a photo of "
+NEGATIVE_PROMPT = "monochrome, lowres, bad anatomy, worst quality, low quality"
+PROMPT_FIELDS = ("prompt_embeds", "negative_prompt_embeds", "pooled_prompt_embeds", "negative_pooled_prompt_embeds")
+
+
+def encode_description(pipe, description, device=None):
+    """The demo's two encode_prompt calls for a garment description: {the four PROMPT_FIELDS, text_embeds_cloth}, each
+    without its batch dimension (the shapes of the TryOnRequest fields)."""
+    pe, npe, ppe, nppe = pipe.encode_prompt(PERSON_PROMPT + description, device=device, num_images_per_prompt=1,
+                                            do_classifier_free_guidance=True, negative_prompt=NEGATIVE_PROMPT)
+    cloth = pipe.encode_prompt([GARMENT_PROMPT + description], device=device, num_images_per_prompt=1,
+                               do_classifier_free_guidance=False, negative_prompt=[NEGATIVE_PROMPT])[0]
+    return dict(prompt_embeds=pe[0], negative_prompt_embeds=npe[0], pooled_prompt_embeds=ppe[0],
+                negative_pooled_prompt_embeds=nppe[0], text_embeds_cloth=cloth[0])
+
+
+def _can_encode(pipe):
+    """Whether encode_prompt can run: tokenizer_2 and text_encoder_2, and the first pair both or neither."""
+    get = lambda n: getattr(pipe, n, None)  # noqa: E731
+    return get("tokenizer_2") is not None and get("text_encoder_2") is not None and \
+        (get("tokenizer") is None) == (get("text_encoder") is None)
+
+
+def _has_garment_image(req):
+    return req.cloth is not None or req.garment_photo is not None
+
+
+def _derived_garment(req):
+    """Whether the garment `req` brings is made by the server (a garment photo or a description)."""
+    return req.garment_photo is not None or req.garment_description is not None
+
+
+def _check_garment_request(req, pipe, source):
+    """Submit-time checks of a request's garment and prompt fields (ValueError). source: the garment's entry (a dict)
+    when it is encoded, the request that brought it when that request still waits, None when `req` brings it."""
+    gid = req.garment_id
+    if req.garment_photo is not None:
+        if req.cloth is not None or req.ip_adapter_image is not None:
+            raise ValueError("garment_photo replaces cloth and ip_adapter_image: give one or the other")
+        from .photo import check_garment
+        check_garment(req.garment_photo)
+    if req.garment_description is not None:
+        if req.text_embeds_cloth is not None:
+            raise ValueError("garment_description replaces text_embeds_cloth: give one or the other")
+        if not isinstance(req.garment_description, str):
+            raise ValueError(f"garment_description must be a str, got {type(req.garment_description).__name__}")
+        if not _can_encode(pipe):
+            raise ValueError("garment_description needs a pipeline with its tokenizers and text encoders")
+    given = sum(getattr(req, f) is not None for f in PROMPT_FIELDS)
+    if given not in (0, len(PROMPT_FIELDS)):
+        raise ValueError(f"give all four prompt embeddings {PROMPT_FIELDS} or none (got {given})")
+    if source is None:
+        if req.garment_photo is None and (req.cloth is None or req.ip_adapter_image is None):
+            raise ValueError(f"garment {gid!r} is new: cloth and ip_adapter_image, or garment_photo, are required")
+        if req.text_embeds_cloth is None and req.garment_description is None:
+            raise ValueError(f"garment {gid!r} is new: text_embeds_cloth or garment_description is required")
+        described = req.garment_description is not None
+    else:
+        described = "prompt_embeds" in source if isinstance(source, dict) else source.garment_description is not None
+    if not given and not described:
+        raise ValueError(f"the request has no prompt embeddings and garment {gid!r} has no garment_description to "
+                         "make them from")
+
+
+def _prompts(req, g):
+    """The request's four prompt embeddings, or its garment's description-derived ones."""
+    if req.prompt_embeds is not None:
+        return [getattr(req, f) for f in PROMPT_FIELDS]
+    return [g[f] for f in PROMPT_FIELDS]
+
+
+class _GarmentFailed(Exception):
+    """A garment made by the server (photo or description) could not be prepared; __cause__ is the error."""
+
+
+def _prepare_garment_photos(photos, height, width):
+    """(entries, failed): photo.prepare_garments of `photos` in one call. If that call raises, each photo is prepared
+    on its own, and the ones that still raise come back in `failed` ({index: exception}, entry None). A library without
+    the kernels raises (NotImplementedError)."""
+    from .photo import prepare_garments
+    if not photos:
+        return [], {}
+    try:
+        return prepare_garments(photos, height, width), {}
+    except NotImplementedError:
+        raise
+    except (ValueError, RuntimeError):
+        entries, failed = [None] * len(photos), {}
+        for i, p in enumerate(photos):
+            try:
+                entries[i] = prepare_garments([p], height, width)[0]
+            except NotImplementedError:
+                raise
+            except (ValueError, RuntimeError) as exc:
+                failed[i] = exc
+        return entries, failed
 
 
 @dataclasses.dataclass
@@ -106,14 +216,23 @@ def _scheduler_installed(pipe, scheduler):
         pipe.scheduler = old
 
 
-def _encode_garment(pipe, src, seed, device, dtype):
+def _encode_garment(pipe, src, seed, device, dtype, prepared=None):
     """ONE posterior sample per garment, from a generator of its own (seeded with the server's seed): the per-request
-    generator must see the same stream whether or not the garment was already known."""
-    cloth = src.cloth[None].to(device=device, dtype=dtype)
+    generator must see the same stream whether or not the garment was already known. prepared: the PreparedGarment of
+    src.garment_photo (its cloth and CLIP pixels replace src's). A garment_description is encoded here, once: the
+    entry then holds its text_embeds_cloth and the four person-prompt embeddings."""
+    cloth = (src.cloth if prepared is None else prepared.cloth)[None].to(device=device, dtype=dtype)
     gen = torch.Generator(device).manual_seed(seed) if seed is not None else None
     latents = pipe._encode_vae_image(cloth, generator=gen)
-    return dict(latents=latents, ip_adapter_image=src.ip_adapter_image[None].to(device),
-                text_embeds_cloth=src.text_embeds_cloth[None].to(device=device, dtype=dtype))
+    ip = src.ip_adapter_image if prepared is None else prepared.clip_pixels
+    g = dict(latents=latents, ip_adapter_image=ip[None].to(device))
+    if src.garment_description is None:
+        g["text_embeds_cloth"] = src.text_embeds_cloth[None].to(device=device, dtype=dtype)
+    else:
+        emb = encode_description(pipe, src.garment_description, device)
+        g["text_embeds_cloth"] = emb.pop("text_embeds_cloth")[None].to(device=device, dtype=dtype)
+        g.update(emb)
+    return g
 
 
 def _check_photo_request(req, height, width):
@@ -250,7 +369,8 @@ class TryOnServer:
     calls the pipeline with its preset's arguments, its scheduler (a private copy) installed for the call. None: one
     preset from num_inference_steps and guidance_scale with the pipeline's scheduler.
     Photo requests (TryOnRequest.photo) whose preparation fails are dropped from their batch, which still runs; their
-    tickets map to the exception in `failed`."""
+    tickets map to the exception in `failed`. A garment made from a garment_photo or a garment_description is prepared
+    when its first batch runs; if that fails, every waiting request of its garment_id goes to `failed`."""
 
     def __init__(self, pipe, height=1024, width=768, num_inference_steps=30, guidance_scale=2.0, max_batch=8, seed=None,
                  garment_cache_bytes=40 << 30, output_type="pt", presets=None, default_preset=None, photo_filter="bicubic"):
@@ -281,9 +401,8 @@ class TryOnServer:
     def submit(self, req: TryOnRequest):
         name = _preset_name(self, req)
         _check_photo_request(req, self.height, self.width)
-        if req.garment_id not in self.garments and all(g != req.garment_id for g, _ in self.queue) and \
-                (req.cloth is None or req.ip_adapter_image is None or req.text_embeds_cloth is None):
-            raise ValueError(f"garment {req.garment_id!r} is new: cloth, ip_adapter_image and text_embeds_cloth are required")
+        g = self.garments.get(req.garment_id)
+        _check_garment_request(req, self.pipe, g if g is not None else self._pending_source(req.garment_id))
         req.ticket = self._next_ticket
         self._next_ticket += 1
         self.queue.setdefault((req.garment_id, name), collections.deque()).append(req)
@@ -305,13 +424,46 @@ class TryOnServer:
         p = self.presets[name]
         return SamplingPreset(None, self.num_inference_steps, self.guidance_scale) if p is None else p
 
+    def _pending_source(self, gid, extra=()):
+        """The waiting request (of `extra` or the queue) that brought garment `gid`: the first one with its image."""
+        cands = [r for r in extra if _has_garment_image(r)]
+        cands += [r for (g, _), q in self.queue.items() if g == gid for r in q if _has_garment_image(r)]
+        return min(cands, key=lambda r: r.ticket) if cands else None
+
     def _garment(self, gid, batch, device, dtype):
+        """The garment's entry, encoded on first use. A garment made from a photo or a description that fails raises
+        _GarmentFailed."""
         g = self.garments.get(gid)
         if g is None:
-            g = _encode_garment(self.pipe, next(r for r in batch if r.cloth is not None), self.seed, device, dtype)
+            src = self._pending_source(gid, batch)
+            try:
+                prepared = None
+                if src.garment_photo is not None:
+                    entries, failed = _prepare_garment_photos([src.garment_photo], self.height, self.width)
+                    if failed:
+                        raise failed[0]
+                    prepared = entries[0]
+                    self.stats["garment_photos_prepared"] += 1
+                g = _encode_garment(self.pipe, src, self.seed, device, dtype, prepared)
+            except NotImplementedError:
+                raise
+            except (ValueError, RuntimeError) as exc:
+                if not _derived_garment(src):
+                    raise
+                raise _GarmentFailed(f"garment {gid!r} could not be prepared") from exc
+            self.stats["descriptions_encoded"] += src.garment_description is not None
             self.garments[gid] = g
             self.stats["garments_encoded"] += 1
         return g
+
+    def _drop_garment(self, gid, batch, exc):
+        """Every waiting request of garment `gid` (`batch` and the queue) fails with `exc`; the id is unknown again."""
+        dropped = list(batch)
+        for key in [k for k in self.queue if k[0] == gid]:
+            dropped += self.queue.pop(key)
+        for r in dropped:
+            self.failed[r.ticket] = exc
+        self.stats["failed"] += len(dropped)
 
     @torch.no_grad()
     def step(self):
@@ -323,9 +475,16 @@ class TryOnServer:
         pipe = self.pipe
         device = pipe._execution_device
         dtype = pipe.unet.dtype
+        try:
+            g = self._garment(gid, batch, device, dtype)
+        except _GarmentFailed as exc:       # the garment's requests are dropped; the server goes on
+            self._drop_garment(gid, batch, exc.__cause__)
+            return {}
         gen = torch.Generator(device).manual_seed(self.seed) if self.seed is not None else None
-        g = self._garment(gid, batch, device, dtype)
         stack = lambda name, dt=None: torch.stack([getattr(r, name) for r in batch]).to(device=device, dtype=dt)  # noqa: E731
+        prompts = [_prompts(r, g) for r in batch]
+        # a request's own tensors may be on the host, a garment's derived ones are on the device
+        prompt = lambda j: torch.stack([p[j].to(device=device, dtype=dtype) for p in prompts])  # noqa: E731
         entries, failed = _prepare_photos_or_drop(batch, self.height, self.width, self.photo_filter)
         if failed:            # dropped from the batch; the rest of it runs
             for i, exc in failed.items():
@@ -351,9 +510,8 @@ class TryOnServer:
         # the pose latents' sample comes from the global generator: seeded around the call (_seeded_global_rng), so a
         # seeded server is reproducible
         with _scheduler_installed(pipe, self._schedulers[name]), _seeded_global_rng(device, self.seed):
-            images = pipe(prompt_embeds=stack("prompt_embeds", dtype), negative_prompt_embeds=stack("negative_prompt_embeds", dtype),
-                          pooled_prompt_embeds=stack("pooled_prompt_embeds", dtype),
-                          negative_pooled_prompt_embeds=stack("negative_pooled_prompt_embeds", dtype),
+            images = pipe(prompt_embeds=prompt(0), negative_prompt_embeds=prompt(1), pooled_prompt_embeds=prompt(2),
+                          negative_pooled_prompt_embeds=prompt(3),
                           num_inference_steps=preset.num_inference_steps, generator=gen, strength=preset.strength,
                           pose_img=person["pose_img"], text_embeds_cloth=g["text_embeds_cloth"], cloth=g["latents"],
                           mask_image=person["mask_image"], image=person["image"], height=self.height,
@@ -422,7 +580,9 @@ class ContinuousTryOnServer:
     kernel (b200vton_cfg_step_mixed_rows) when presets need it, or, in pool mode, b200vton_attention_rows
     (NotImplementedError naming the symbol). An unknown preset name is refused at submit (ValueError).
     Photo requests (TryOnRequest.photo) are prepared at admission; one whose preparation fails is dropped from the queue
-    without taking a slot, and its ticket maps to the exception in `failed`."""
+    without taking a slot, and its ticket maps to the exception in `failed`. The new garments of an admission made from
+    a garment_photo or a garment_description are prepared there, their photos in one prepare_garments call; a garment
+    that fails takes every waiting request of its garment_id to `failed`."""
 
     def __init__(self, pipe, height=1024, width=768, slots=4, num_inference_steps=30, guidance_scale=2.0, seed=None,
                  output_type="pt", eta=0.0, garment_kv_bytes=None, presets=None, default_preset=None,
@@ -457,18 +617,17 @@ class ContinuousTryOnServer:
         self.last_latents = {}                       # ticket -> final latents of the requests the last step() finished
         self._next_ticket = 0
         self.stats = collections.Counter()
-        self.failed = {}                             # ticket -> exception: photo requests whose preparation failed
+        self.failed = {}                             # ticket -> exception: requests whose photo or garment failed
+        self._prepared_garments = {}                 # garment_id -> PreparedGarment made at this admission
 
     # ---------------------------------------------------------------------------------------------
     def submit(self, req: TryOnRequest):
         _preset_name(self, req)
         _check_photo_request(req, self.height, self.width)
-        known = req.garment_id in self.garments or any(r.garment_id == req.garment_id for r in self.waiting) or any(
-            e is not None and e["req"].garment_id == req.garment_id for e in self.slots)
-        if not known:
-            if req.cloth is None or req.ip_adapter_image is None or req.text_embeds_cloth is None:
-                raise ValueError(f"garment {req.garment_id!r} is new: cloth, ip_adapter_image and text_embeds_cloth are "
-                                 "required")
+        g = self.garments.get(req.garment_id)
+        source = g if g is not None else self._pending_source(req.garment_id)
+        _check_garment_request(req, self.pipe, source)
+        if source is None and req.garment_photo is None:       # a garment photo is resized to the server's size
             vsf = self.pipe.vae_scale_factor
             size = (req.cloth.shape[-2] // vsf, req.cloth.shape[-1] // vsf)
             if size != self.latent_size:
@@ -585,17 +744,72 @@ class ContinuousTryOnServer:
         self.T = T_max
         self._configured = True
 
+    def _pending_source(self, gid):
+        """The waiting request that brought garment `gid`: the first one with its image."""
+        return next((r for r in self.waiting if r.garment_id == gid and _has_garment_image(r)), None)
+
     def _garment(self, req, device, dtype):
+        """The garment's entry, encoded on first use (with the PreparedGarment of this admission when it has a photo).
+        A garment made from a photo or a description that fails raises _GarmentFailed."""
         g = self.garments.get(req.garment_id)
         if g is None:
-            src = req if req.cloth is not None else next(
-                r for r in self.waiting if r.garment_id == req.garment_id and r.cloth is not None)
-            g = _encode_garment(self.pipe, src, self.seed, device, dtype)
-            emb = self.pipe.prepare_ip_adapter_image_embeds(g["ip_adapter_image"], device, 1)
-            g["image_embeds"] = self.pipe.unet.encoder_hid_proj(emb).to(dtype)         # Resampler, once per garment
+            src = req if _has_garment_image(req) else self._pending_source(req.garment_id)
+            try:
+                prepared = self._prepared_garments.pop(req.garment_id, None)
+                if prepared is None and src.garment_photo is not None:
+                    entries, failed = _prepare_garment_photos([src.garment_photo], self.height, self.width)
+                    if failed:
+                        raise failed[0]
+                    prepared = entries[0]
+                    self.stats["garment_photos_prepared"] += 1
+                g = _encode_garment(self.pipe, src, self.seed, device, dtype, prepared)
+                emb = self.pipe.prepare_ip_adapter_image_embeds(g["ip_adapter_image"], device, 1)
+                g["image_embeds"] = self.pipe.unet.encoder_hid_proj(emb).to(dtype)         # Resampler, once per garment
+            except NotImplementedError:
+                raise
+            except (ValueError, RuntimeError) as exc:
+                if not _derived_garment(src):
+                    raise
+                raise _GarmentFailed(f"garment {req.garment_id!r} could not be prepared") from exc
+            self.stats["descriptions_encoded"] += src.garment_description is not None
             self.garments[req.garment_id] = g
             self.stats["garments_encoded"] += 1
         return g
+
+    def _encode_new_garments(self, heads, device, dtype):
+        """Encodes the new garments of `heads` that the server makes itself (a photo or a description), their photos
+        in one prepare_garments call. A garment that fails takes every waiting request of its id into `failed`, and the
+        id is unknown again. Returns whether any was dropped (the heads changed)."""
+        new = {}
+        for r in heads:
+            if r.garment_id not in self.garments and r.garment_id not in new:
+                src = self._pending_source(r.garment_id)
+                if src is not None and _derived_garment(src):
+                    new[r.garment_id] = src
+        photo = [gid for gid, src in new.items() if src.garment_photo is not None]
+        entries, failed = _prepare_garment_photos([new[gid].garment_photo for gid in photo], self.height, self.width)
+        dropped = {photo[j]: exc for j, exc in failed.items()}
+        for gid, e in zip(photo, entries):
+            if e is not None:
+                self._prepared_garments[gid] = e
+                self.stats["garment_photos_prepared"] += 1
+        for gid, src in new.items():
+            if gid not in dropped:
+                try:
+                    self._garment(src, device, dtype)
+                except _GarmentFailed as exc:
+                    dropped[gid] = exc.__cause__
+        for gid, exc in dropped.items():
+            self._prepared_garments.pop(gid, None)
+            keep = collections.deque()
+            for r in self.waiting:
+                if r.garment_id == gid:
+                    self.failed[r.ticket] = exc
+                    self.stats["failed"] += 1
+                else:
+                    keep.append(r)
+            self.waiting = keep
+        return bool(dropped)
 
     def _prepare_request(self, req, gen, entry=None):
         """The pipeline's own preparation of one person (batch 1, the request's preset and its scheduler installed):
@@ -612,12 +826,11 @@ class ContinuousTryOnServer:
         device, dtype = pipe._execution_device, pipe.unet.dtype
         do_cfg = pipe.do_classifier_free_guidance
         H, W = self.height, self.width
+        prompts = [p[None].to(device=device, dtype=dtype) for p in _prompts(req, self.garments.get(req.garment_id))]
         pe, npe, ppe, nppe = pipe.encode_prompt(
             prompt=None, device=device, num_images_per_prompt=1, do_classifier_free_guidance=do_cfg,
-            prompt_embeds=req.prompt_embeds[None].to(device=device, dtype=dtype),
-            negative_prompt_embeds=req.negative_prompt_embeds[None].to(device=device, dtype=dtype),
-            pooled_prompt_embeds=req.pooled_prompt_embeds[None].to(device=device, dtype=dtype),
-            negative_pooled_prompt_embeds=req.negative_pooled_prompt_embeds[None].to(device=device, dtype=dtype))
+            prompt_embeds=prompts[0], negative_prompt_embeds=prompts[1], pooled_prompt_embeds=prompts[2],
+            negative_pooled_prompt_embeds=prompts[3])
         image, mask_image, pose_img = _person_inputs(req, entry)
         init_image, mask, masked_image, mask_latent = pipe._preprocess_image_mask(
             image[None].to(device=device), mask_image[None].to(device=device), None, H, W)
@@ -661,6 +874,8 @@ class ContinuousTryOnServer:
         while free and self.waiting:       # again when a dropped request left a slot free
             n = min(len(free), len(self.waiting))
             heads = [self.waiting[i] for i in range(n)]
+            if self._encode_new_garments(heads, device, dtype):
+                continue                   # garments were dropped with their requests: take the heads again
             entries, failed = _prepare_photos_or_drop(heads, self.height, self.width, self.photo_filter)
             slots = iter(free)
             for i, entry in enumerate(entries):

@@ -370,6 +370,22 @@ typedef struct b200vton_paste_desc {
 } b200vton_paste_desc;
 int b200vton_paste_u8(const b200vton_paste_desc* descs, const void* descs_dev, int n, void* stream);
 
+/* b200vton_clip_pixels_u8: CLIPImageProcessor's centre crop, rescale and normalize (INTEGRATION.md, "Garment photos and
+ * descriptions") of a batch of uint8 HWC RGB images already resampled to the CLIP size (short side 224), in one launch:
+ *   out[j][c][y][x] = table[c * 256 + src_j[crop_y + y][crop_x + x][c]],   0 <= x, y < 224,
+ * out fp32 NCHW [n, 3, 224, 224]. table: 3 x 256 fp32 in device memory (per channel, float32((float64(v) / 255 - mean)
+ * / std) as transformers computes it). Each descriptor has its own size and crop origin; the 224 x 224 crop must lie
+ * inside the image. descs (host) is checked; descs_dev is the same table in device memory, read by the kernel.
+ * n <= 4096. */
+#define B200VTON_CLIP_SIZE 224
+typedef struct b200vton_clip_desc {
+  const uint8_t* src;
+  int64_t src_pitch;  /* bytes per row */
+  int32_t src_w, src_h, crop_x, crop_y;
+} b200vton_clip_desc;
+int b200vton_clip_pixels_u8(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table,
+                            float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
