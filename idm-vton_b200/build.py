@@ -10,7 +10,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200vton.so")
-SOURCES = ["host.cu", "gemm.cu", "attn.cu", "norm_f32.cu", "vae_f32.cu", "norm.cu", "elementwise.cu", "photo.cu", "capi.cu"]
+SOURCES = ["host.cu", "gemm.cu", "attn.cu", "norm_f32.cu", "vae_f32.cu", "norm.cu", "elementwise.cu", "photo.cu",
+           "freeu.cu", "capi.cu"]
 HEADERS = ["common.cuh", "gemm_common.cuh", "wgmma.cuh", "host.h", os.path.join("..", "..", "include", "b200vton.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -84,6 +84,8 @@ int resample_u8_impl(const b200vton_resample_desc* descs, const void* descs_dev,
 int paste_u8_impl(const b200vton_paste_desc* descs, const void* descs_dev, int n, cudaStream_t stream);
 int clip_pixels_u8_impl(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table, float* out,
                         cudaStream_t stream);
+int freeu_impl(void* hidden, int Ch, const void* skip, void* skip_out, int Cs, int B, int H, int W, float b, float s,
+               cudaStream_t stream);
 }  // namespace vton
 
 #define S(stream) static_cast<cudaStream_t>(stream)
@@ -316,6 +318,11 @@ int b200vton_paste_u8(const b200vton_paste_desc* descs, const void* descs_dev, i
 int b200vton_clip_pixels_u8(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table,
                             float* out, void* stream) {
   return vton::clip_pixels_u8_impl(descs, descs_dev, n, table, out, S(stream));
+}
+
+int b200vton_freeu_nhwc(void* hidden, int Ch, const void* skip, void* skip_out, int Cs, int B, int H, int W, float b,
+                        float s, void* stream) {
+  return vton::freeu_impl(hidden, Ch, skip, skip_out, Cs, B, H, W, b, s, S(stream));
 }
 
 }  // extern "C"

@@ -262,6 +262,12 @@ def garment_kv_format(tryon):
     return getattr(tryon, "garment_kv_format", "fp16")
 
 
+def freeu_setting(tryon):
+    """(s1, s2, b1, b2) when the try-on engine runs FreeU in its forward (UNetEngine.freeu_active), else None."""
+    active = getattr(tryon, "freeu_active", None)
+    return None if active is None else active()
+
+
 def new_garment_kv(tryon, rows, ng, blk):
     """Storage for `rows` rows of one try-on block's hoisted garment K/V in garment_kv_format(tryon): fp16
     [rows, Ng, 2C], or a GarmentKV8."""
@@ -394,11 +400,11 @@ class _CapturedStep:
     kinds = None                 # per-sample kind codes of the mixed-kind step (SlotDenoiser.configure_presets)
 
     def _signature(self):
-        """What a captured step bakes in: the kernel selection and the address, shape and dtype of every buffer the
-        graph reads or writes (not of those it allocates while capturing, such as eps)."""
+        """What a captured step bakes in: the kernel selection, the try-on UNet's FreeU values, and the address, shape and
+        dtype of every buffer the graph reads or writes (not of those it allocates while capturing, such as eps)."""
         gkv_pre = self._gkv_pre()
         garment = (self.x_g, self.t_g, self.ctx_g) if gkv_pre is None else gkv_pre
-        return (self.kind, self.rescale, self.do_cfg, gkv_pre is not None) + _describe(
+        return (self.kind, self.rescale, self.do_cfg, gkv_pre is not None, freeu_setting(self.tryon)) + _describe(
             [self.latents, self.latents_next, self.noise, self.x0_prev, self.x_t, self.t_t, self.coef, self.scale,
              self.kinds, self.aug, self.ctx_t, garment])
 

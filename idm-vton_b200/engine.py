@@ -85,6 +85,12 @@ class _GarmentDone(Exception):
     """Raised inside the garment UNet's launch sequence once the last garment feature has been exported."""
 
 
+def active_freeu(freeu):
+    """The FreeU values (s1, s2, b1, b2) that run, or None. As in the reference's up blocks
+    (src/unet_block_hacked_tryon.py:2322-2327), FreeU runs only if all four are truthy: a 0 switches it off."""
+    return None if freeu is None or not all(freeu) else tuple(freeu)
+
+
 class UNetEngine:
     """Launch sequence of one SDXL-family UNet (DownBlock2D, 2x CrossAttnDownBlock2D, mid, 2x CrossAttnUpBlock2D,
     UpBlock2D) over NHWC fp16 buffers. kind = "tryon" (src/unet_hacked_tryon.py) or "garment"
@@ -113,6 +119,8 @@ class UNetEngine:
         # format of the hoisted garment K/V the denoisers keep for this (try-on) UNet: "fp16" or "fp8" (lib.GarmentKV8);
         # set by UNet2DConditionModel.set_garment_kv_precision
         self.garment_kv_format = "fp16"
+        # FreeU of the try-on UNet's up stages 0 and 1: None or (s1, s2, b1, b2), set by UNet2DConditionModel.enable_freeu
+        self.freeu = None
         self._kv_scratch = None
         if self.fp8:
             for name in ("b200vton_layernorm_e4m3", "b200vton_gemm_e4m3"):
@@ -246,6 +254,11 @@ class UNetEngine:
 
     def blocks(self):
         return [b for t in self.t2ds() for b in t.blocks]
+
+    def freeu_active(self):
+        """(s1, s2, b1, b2) when FreeU runs in this UNet's forward (the try-on UNet only), else None (also for an engine
+        object made without __init__, which has no `freeu`)."""
+        return active_freeu(getattr(self, "freeu", None)) if self.kind == "tryon" else None
 
     # -------------------------------------------------------------------------------------------
     # step-invariant precompute (once per request): cross-attention K/V, aug_emb (SURVEY.md App. D.5)
@@ -462,9 +475,16 @@ class UNetEngine:
         x = self._resnet(self.mid_res[0], x, None, temb_all)
         x = self._t2d(self.mid_attn, x, state)
         x = self._resnet(self.mid_res[1], x, None, temb_all)
+        freeu = self.freeu_active()
         for i, lvl in enumerate(self.up):
             for j, r in enumerate(lvl["res"]):
-                x = self._resnet(r, x, skips.pop(), temb_all)
+                skip = skips.pop()
+                if freeu is not None and i < 2:
+                    # apply_freeu(resolution_idx=i) before the resnet's cat: stage 0 takes (b1, s1), stage 1 (b2, s2);
+                    # x and skip are this step's own buffers, so both are rewritten in place
+                    s1, s2, b1, b2 = freeu
+                    L.freeu(x, skip, b1 if i == 0 else b2, s1 if i == 0 else s2)
+                x = self._resnet(r, x, skip, temb_all)
                 if lvl["attn"]:
                     x = self._t2d(lvl["attn"][j], x, state)
             if lvl["up"] is not None:

@@ -50,7 +50,7 @@ SIGNATURES = {
 # Entry points bound only when the loaded library exports them (added without an ABI version change): the per-sample
 # step kernels of the continuous-batching denoiser (per kind, and mixed-kind for sampling presets), the FP8 linears,
 # the per-sample-row attention of its pool mode, the FP8 garment K/V (quantizer and attention) and the full-resolution
-# photo kernels (resampler, paste-back and the garment's CLIP pixels).
+# photo kernels (resampler, paste-back and the garment's CLIP pixels) and FreeU.
 # `has_symbol` tells whether a binding can use them.
 OPTIONAL_SIGNATURES = {
     "b200vton_cfg_ddpm_step_rows": [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp],
@@ -67,6 +67,7 @@ OPTIONAL_SIGNATURES = {
     "b200vton_resample_u8": [_vp, _vp, _i, _vp, _i64, _vp, _i64, _vp],
     "b200vton_paste_u8": [_vp, _vp, _i, _vp],
     "b200vton_clip_pixels_u8": [_vp, _vp, _i, _vp, _vp, _vp],
+    "b200vton_freeu_nhwc": [_vp, _i, _vp, _vp, _i, _i, _i, _i, _f, _f, _vp],
 }
 _present = set()
 
@@ -949,3 +950,25 @@ def clip_pixels_u8(descs, table, out):
     arr = (ClipDesc * len(descs))(*descs)
     dev = _descs_to_device(arr, out.device)
     _check(fn(arr, _p(dev), len(descs), _p(table), _p(out), _stream()), "b200vton_clip_pixels_u8")
+
+
+def freeu(hidden, skip, b, s, out=None):
+    """FreeU before one up-stage resnet (diffusers `apply_freeu`): scales the first half of hidden's channels by b in
+    place (fp16(float(h) * b)) and writes fourier_filter(skip, threshold=1, scale=s) to `out`, or in place into skip
+    when out is None. hidden [B,H,W,Ch] and skip [B,H,W,Cs]: contiguous NHWC fp16 CUDA tensors at the same B, H, W.
+    Returns the filtered skip."""
+    fn = _optional("b200vton_freeu_nhwc")
+    _f16(hidden, "hidden"); _f16(skip, "skip"); _f16(out, "out")
+    if hidden.ndim != 4 or skip.ndim != 4 or hidden.shape[:3] != skip.shape[:3]:
+        raise ValueError(f"freeu: hidden {tuple(hidden.shape)} and skip {tuple(skip.shape)} must be [B,H,W,C] at the "
+                         "same B, H, W")
+    if not hidden.is_contiguous() or not skip.is_contiguous():
+        raise ValueError("freeu: hidden and skip must be contiguous")
+    if out is None:
+        out = skip
+    elif out.shape != skip.shape or not out.is_contiguous():
+        raise ValueError(f"freeu: out must be a contiguous tensor of skip's shape {tuple(skip.shape)}")
+    B, H, W, Ch = hidden.shape
+    rc = fn(_p(hidden), Ch, _p(skip), _p(out), skip.shape[3], B, H, W, float(b), float(s), _stream())
+    _check(rc, "b200vton_freeu_nhwc")
+    return out

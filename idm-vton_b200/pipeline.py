@@ -152,6 +152,19 @@ class StableDiffusionXLInpaintPipeline:
             if self.garment_cache is not None:
                 self.garment_cache.clear()
 
+    def enable_freeu(self, s1: float, s2: float, b1: float, b2: float):
+        """FreeU on the try-on UNet (src/tryon_pipeline.py:1096-1116, https://arxiv.org/abs/2309.11497): s1 / s2 scale the
+        lowest frequencies of the skip features of the first / second up stage, b1 / b2 the first half of their backbone
+        channels.
+        FreeU runs only while all four values are non-zero. The garment UNet is not affected."""
+        if not hasattr(self, "unet"):
+            raise ValueError("The pipeline must have `unet` for using FreeU.")
+        self.unet.enable_freeu(s1=s1, s2=s2, b1=b1, b2=b2)
+
+    def disable_freeu(self):
+        """Disables FreeU (src/tryon_pipeline.py:1118-1121)."""
+        self.unet.disable_freeu()
+
     def register_to_config(self, **kw):
         for k, v in kw.items():
             setattr(self.config, k, v)

@@ -21,6 +21,7 @@ from typing import Any, Hashable, Optional
 import torch
 
 from .denoise import GarmentKVCache
+from .engine import active_freeu
 
 
 @dataclasses.dataclass
@@ -535,6 +536,11 @@ class TryOnServer:
         return out
 
 
+def _freeu(pipe):
+    """The FreeU values the pipeline's try-on UNet runs with (enable_freeu, all four non-zero), or None."""
+    return active_freeu(getattr(pipe.unet, "freeu", None))
+
+
 class ContinuousTryOnServer:
     """Continuous batching: requests join and leave the denoise batch at every step (denoise.SlotDenoiser).
 
@@ -870,6 +876,7 @@ class ContinuousTryOnServer:
         if not getattr(self, "_configured", False):
             self._configure()
             self._kv_format = fmt
+            self._freeu = _freeu(self.pipe)
         device, dtype = self.pipe._execution_device, self.pipe.unet.dtype
         while free and self.waiting:       # again when a dropped request left a slot free
             n = min(len(free), len(self.waiting))
@@ -928,9 +935,21 @@ class ContinuousTryOnServer:
             return latents
         return self.pipe._postprocess(self.pipe._decode_latents(latents), self.output_type)
 
+    def _check_freeu(self):
+        """The try-on UNet's FreeU setting is read at configure. A request must not run part of its steps with other
+        values, so a change while requests run raises; a change while the server is idle re-configures. The garment
+        UNet does not run FreeU, so garment latents, K/V and pool pages stay valid."""
+        if not getattr(self, "_configured", False) or _freeu(self.pipe) == self._freeu:
+            return
+        if any(e is not None for e in self.slots):
+            raise RuntimeError(f"the pipeline's FreeU setting changed to {_freeu(self.pipe)} while requests run with "
+                               f"{self._freeu}: change it when the server is idle")
+        self._configured = False
+
     @torch.no_grad()
     def step(self, use_graph=True):
         """Admits, runs one denoise step, decodes and frees the slots that finished. Returns {ticket: image}."""
+        self._check_freeu()
         self._admit()
         active = [s for s, e in enumerate(self.slots) if e is not None]
         if not active:

@@ -399,6 +399,7 @@ class UNet2DConditionModel(_UNetBase):
     def __init__(self, cfg=None, state_dict=None, device="cpu", dtype=torch.float16):
         super().__init__(cfg or SDXL_TRYON, state_dict, device, dtype)
         self._garment_kv_precision = "fp16"
+        self._freeu = None
 
     GARMENT_KV_PRECISIONS = ("fp16", "fp8")
 
@@ -419,7 +420,28 @@ class UNet2DConditionModel(_UNetBase):
     def engine(self):
         eng = super().engine()
         eng.garment_kv_format = self._garment_kv_precision
+        eng.freeu = self._freeu
         return eng
+
+    @property
+    def freeu(self):
+        """(s1, s2, b1, b2) set by enable_freeu, or None."""
+        return self._freeu
+
+    def enable_freeu(self, s1, s2, b1, b2):
+        """FreeU (https://arxiv.org/abs/2309.11497, src/unet_hacked_tryon.py:938-959): before every resnet of up stage 0
+        the first half of the backbone channels is scaled by b1 and the skip feature's lowest frequencies by s1
+        (stage 1: b2, s2). As in the reference, FreeU runs only while all four values are non-zero. The weights are not
+        re-packed; a captured denoise step is re-captured at its next run."""
+        self._freeu = tuple(None if v is None else float(v) for v in (s1, s2, b1, b2))
+        if self._engine is not None:
+            self._engine.freeu = self._freeu
+
+    def disable_freeu(self):
+        """Switches FreeU off (src/unet_hacked_tryon.py:961-967)."""
+        self._freeu = None
+        if self._engine is not None:
+            self._engine.freeu = None
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, timestep_cond=None,
@@ -468,6 +490,11 @@ class UNet2DConditionModelGarment(_UNetBase):
 
     def __init__(self, cfg=None, state_dict=None, device="cpu", dtype=torch.float16):
         super().__init__(cfg or SDXL_GARMENT, state_dict, device, dtype)
+
+    def enable_freeu(self, s1, s2, b1, b2):
+        raise NotImplementedError("FreeU on the garment UNet is not supported: it would change the garment features, "
+                                  "so the hoisted garment K/V, the GarmentKVCache keys and the pool pages would all "
+                                  "depend on it. The reference pipeline's enable_freeu only touches the try-on UNet.")
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, timestep_cond=None,

@@ -386,6 +386,17 @@ typedef struct b200vton_clip_desc {
 int b200vton_clip_pixels_u8(const b200vton_clip_desc* descs, const void* descs_dev, int n, const float* table,
                             float* out, void* stream);
 
+/* b200vton_freeu_nhwc: FreeU (diffusers `apply_freeu`, https://arxiv.org/abs/2309.11497) before one resnet of the
+ * try-on UNet's up stage 0 or 1 (src/unet_block_hacked_tryon.py:2322-2344,2458-2480), in one launch:
+ *   hidden[..., c] = fp16(float(hidden[..., c]) * b) for c < Ch / 2, in place (channels Ch / 2.. keep their bits);
+ *   skip_out = fourier_filter(skip, threshold=1, scale=s): the 2-D spectrum of every (sample, channel) plane times s at
+ *   the frequencies {0, -1} along each axis ({0} along an axis of size 1), computed in closed form in fp32 from the
+ *   fp16 input (7 sums per channel in a fixed order, then one pass) and rounded to fp16 once.
+ * hidden [B,H,W,Ch], skip / skip_out [B,H,W,Cs], NHWC fp16, contiguous, 16-byte aligned; Ch % 8 == 0, Cs % 8 == 0.
+ * skip_out may be skip (in place) or must not overlap it; hidden may overlap neither. */
+int b200vton_freeu_nhwc(void* hidden, int Ch, const void* skip, void* skip_out, int Cs, int B, int H, int W, float b,
+                        float s, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
