@@ -268,12 +268,13 @@ def freeu_setting(tryon):
     return None if active is None else active()
 
 
-def new_garment_kv(tryon, rows, ng, blk):
+def new_garment_kv(tryon, rows, ng, blk, device=None):
     """Storage for `rows` rows of one try-on block's hoisted garment K/V in garment_kv_format(tryon): fp16
-    [rows, Ng, 2C], or a GarmentKV8."""
+    [rows, Ng, 2C], or a GarmentKV8. device: the engine's by default (the host tier passes "cpu")."""
+    device = tryon.device if device is None else device
     if garment_kv_format(tryon) == "fp8":
-        return GarmentKV8.empty(rows, ng, blk.c, tryon.device)
-    return torch.empty((rows, ng, 2 * blk.c), dtype=torch.float16, device=tryon.device)
+        return GarmentKV8.empty(rows, ng, blk.c, device)
+    return torch.empty((rows, ng, 2 * blk.c), dtype=torch.float16, device=device)
 
 
 def garment_kv_bytes_per_step(tryon, hg, wg, fmt=None):
@@ -306,6 +307,65 @@ def kv_map(kv, fn):
 
 def kv_parts(kv):
     return tuple(kv) if isinstance(kv, GarmentKV8) else (kv,)
+
+
+def copy_kv_rows(dst, d0, src, s0, n=1):
+    """dst[d0:d0 + n] = src[s0:s0 + n] for one block's hoisted garment K/V (the fp16 tensor, or the e4m3 rows and the
+    int8 exponents of a GarmentKV8), enqueued on the current stream: one cudaMemcpyAsync per part, the rows being
+    contiguous. Between page-locked host memory and the device the host does not wait for it. Returns the bytes."""
+    nbytes = 0
+    for d, s in zip(kv_parts(dst), kv_parts(src)):
+        rows = s[s0:s0 + n]
+        d[d0:d0 + n].copy_(rows, non_blocking=True)
+        nbytes += rows.numel() * rows.element_size()
+    return nbytes
+
+
+def _host_register(t):
+    """Page-locks the storage of CPU tensor t (cudaHostRegister); False when CUDA refuses."""
+    return int(torch.cuda.cudart().cudaHostRegister(t.data_ptr(), t.numel() * t.element_size(), 0)) == 0
+
+
+def _host_unregister(t):
+    torch.cuda.cudart().cudaHostUnregister(t.data_ptr())
+
+
+class HostGarmentKV:
+    """Q pages of hoisted garment K/V in page-locked host memory, in the format of the device pool: per try-on block one
+    fp16 [Q*T_page, Ng, 2C] tensor, or a GarmentKV8 of Q*T_page rows (e4m3 rows and int8 exponents); page q = rows
+    q*T_page .. q*T_page + T_page - 1. The tensors are plain CPU tensors page-locked with cudaHostRegister: torch's
+    pin_memory goes through its caching host allocator, which rounds every allocation up to a power of two (a 9.44 GB
+    page could pin 16 GB). There is no pageable fallback: a failed allocation raises RuntimeError naming the bytes.
+    release() unregisters them; it must come before the tensors are dropped."""
+
+    def __init__(self, tryon, pages, T_page, h, w):
+        self.Q, self.T_page = int(pages), int(T_page)
+        self.bytes = self.Q * self.T_page * garment_kv_bytes_per_step(tryon, h, w)
+        self.blocks, self._locked = [], []
+        try:
+            for b, ng in zip(tryon.blocks(), garment_tokens(tryon, h, w)):
+                kv = new_garment_kv(tryon, self.Q * self.T_page, ng, b, device="cpu")
+                for t in kv_parts(kv):
+                    if not _host_register(t):
+                        raise RuntimeError(f"cudaHostRegister refused {t.numel() * t.element_size()} bytes")
+                    self._locked.append(t)
+                self.blocks.append(kv)
+        except (RuntimeError, MemoryError) as exc:
+            self.release()
+            raise RuntimeError(f"the garment K/V host tier could not allocate and page-lock {self.bytes} bytes "
+                               f"({self.Q} pages of {self.bytes // self.Q} bytes) of host memory: {exc}") from exc
+
+    def release(self):
+        """Unregisters every page-locked tensor (idempotent); the tier holds nothing afterwards."""
+        while self._locked:
+            _host_unregister(self._locked.pop())
+        self.blocks = []
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:       # interpreter shutdown: CUDA may be gone, and the process releases everything
+            pass
 
 
 def hoisted_garment_kv(tryon, garment, x_g, ctx_g, t_table, t0, t1, chunk, out):
@@ -699,6 +759,14 @@ class SlotDenoiser(_CapturedStep):
         and the timesteps. The step is the try-on UNet only: slot s reads row page(s)*T + step(s) of the pool through
         b200vton_attention_rows, and an idle slot reads row -1, the zero-K/V closed form (no K/V traffic, and no
         unwritten memory is ever read). The caller (ContinuousTryOnServer) decides which garment is in which page.
+      * pages=P, host_pages=Q (pool mode with a host tier): Q more pages in page-locked host memory (HostGarmentKV),
+        and 2S more rows at the end of every block's pool tensor, a ring of two rows per slot from R = P*T_page on.
+        write_through(p, q) copies a filled device page to host page q on a side stream; a refill of device page p
+        waits for that copy on the device. A slot admitted with host_page=q streams: at step i it reads ring row
+        R + 2s + (i & 1). Its first row is copied at admission, before the next replay. After each replay the side
+        stream copies the next row of every streaming slot into its other ring row, once the step that last read that
+        row (the previous replay) is done, and the next replay waits for those copies. Only CUDA events order the two
+        streams; the row table is data, so the captured step is the same graph.
 
     Sampling presets (configure_presets): the slots may follow different StepPlans (scheduler, step count, strength,
     guidance scale, DDPM guidance rescale). Their rows share one table with a kind code per row, a slot names (plan,
@@ -712,7 +780,7 @@ class SlotDenoiser(_CapturedStep):
     ROWS = True
     rescale = False              # refused by configure (the rescale kernel reads one row); per row in configure_presets
 
-    def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots, pages=None):
+    def __init__(self, tryon: UNetEngine, garment: UNetEngine, slots, pages=None, host_pages=None):
         self.tryon, self.garment = tryon, garment
         self.L = tryon.L
         self.device = tryon.device
@@ -720,9 +788,19 @@ class SlotDenoiser(_CapturedStep):
         self.P = None if pages is None else int(pages)
         if self.P is not None and self.P < self.S:
             raise ValueError(f"pool mode needs at least one garment K/V page per slot: {self.P} pages for {self.S} slots")
+        self.Q = None if host_pages is None else int(host_pages)
+        if self.Q is not None and (self.P is None or self.Q < 1):
+            raise ValueError(f"a host tier of {self.Q} garment K/V pages needs pool mode (pages=P) and at least one page")
         self.garment_chunk = default_garment_chunk(1)
         self.page = [None] * self.S                 # pool mode: the page each slot's request reads
+        self.host_page = [None] * self.S            # host tier: the host page a streaming slot reads
+        self.host = None
         self.pool = None
+        self._side = None                           # host tier: the copy stream and its events (made at first use)
+        self._page_rows = {}                        # device page -> rows its last fill wrote
+        self._page_copied = {}                      # device page -> event of its last write-through
+        self._host_written = {}                     # host page -> event of its last write-through
+        self._streamed = [0, 0]                     # rows and bytes copied into the ring since take_streamed()
         self._key = None
         self.ctx_t = None
         self.plans = self.kind_table = None         # configure_presets: the plans and the kind of every table row
@@ -804,7 +882,6 @@ class SlotDenoiser(_CapturedStep):
         key = (S, h, w, self.do_cfg, self.kind) + (() if self.P is None else (self.P, self.T_page,
                                                                                garment_kv_format(self.tryon)))
         if key != self._key:
-            self._key = key
             self.ctx_t = self.ctx_g = self.aug = None
             self.latents = torch.zeros((S, 4, h, w), dtype=f16, device=dev)
             self.latents_next = torch.zeros_like(self.latents)
@@ -817,15 +894,23 @@ class SlotDenoiser(_CapturedStep):
             else:
                 # allocated once (the old pool is released first); every page is written by fill_page before a slot's
                 # row names it
+                self.release_host()
+                self._page_rows.clear()
                 self.x_g = self.t_g = self.pool = None
-                self.pool = [new_garment_kv(self.tryon, self.P * self.T_page, ng, b)
+                if self.Q is not None:         # host first: a failed page-lock raises before the device pool grows
+                    self.host = HostGarmentKV(self.tryon, self.Q, self.T_page, h, w)
+                self.ring = self.P * self.T_page
+                ring_rows = 0 if self.Q is None else 2 * S
+                self.pool = [new_garment_kv(self.tryon, self.ring + ring_rows, ng, b)
                              for b, ng in zip(self.tryon.blocks(), garment_tokens(self.tryon, h, w))]
                 self.rows = torch.full((S,), -1, dtype=torch.int32, device=dev)
                 self.page = [None] * S
+                self.host_page = [None] * S
             self.t_t = torch.zeros(self.Bt, dtype=f32, device=dev)
             self.coef = torch.zeros((S, 8), dtype=f32, device=dev)
             self.scale = torch.ones(S, dtype=f32, device=dev)
             self.kinds = torch.zeros(S, dtype=torch.int32, device=dev) if self.kind == "mixed" else None
+            self._key = key                    # last: a failed allocation leaves the key to be allocated again
 
     def gather(self, steps):
         """steps: per slot, the step index of its request or None (idle); after configure_presets, (plan index, step
@@ -852,15 +937,25 @@ class SlotDenoiser(_CapturedStep):
         if self.kind_table is not None:
             torch.index_select(self.kind_table, 0, idx, out=self.kinds)
         if self.P is not None:
-            # pool mode: slot s reads row page(s) * T_page + step(s) of the pool, an idle slot row -1 (zero K/V)
-            rows = []
-            for s, i in enumerate(step_of):
-                if i is not None and self.page[s] is None:
-                    raise ValueError(f"slot {s} is at step {i} but holds no garment K/V page")
-                rows.append(-1 if i is None else self.page[s] * self.T_page + int(i))
-            if any(not -1 <= r < self.P * self.T_page for r in rows):
-                raise ValueError(f"garment K/V rows {rows} outside [-1, {self.P * self.T_page})")
-            self.rows.copy_(torch.tensor(rows, dtype=torch.int32))
+            self.rows.copy_(torch.tensor(self.kv_rows(step_of), dtype=torch.int32))
+
+    def kv_rows(self, step_of):
+        """Pool mode: the pool row of every slot at its step index (None: idle). Slot s reads row page(s) * T_page +
+        step(s); streaming from the host tier, ring row P * T_page + 2s + (step & 1); idle, row -1 (zero K/V)."""
+        rows, streaming = [], []
+        for s, i in enumerate(step_of):
+            if i is None:
+                rows.append(-1)
+            elif self.host_page[s] is not None:
+                rows.append(self.ring + 2 * s + (int(i) & 1))
+                streaming.append(s)
+            elif self.page[s] is None:
+                raise ValueError(f"slot {s} is at step {i} but holds no garment K/V page")
+            else:
+                rows.append(self.page[s] * self.T_page + int(i))
+        if any(not -1 <= r < self.ring for s, r in enumerate(rows) if s not in streaming):   # the device pages' rows
+            raise ValueError(f"garment K/V rows {rows} outside [-1, {self.ring})")
+        return rows
 
     def fill_page(self, p, cloth_latents, text_embeds_cloth, t_table=None):
         """Pool mode: writes the garment K/V of all T steps of one garment (cloth_latents [1,4,h,w], text_embeds_cloth
@@ -885,6 +980,10 @@ class SlotDenoiser(_CapturedStep):
             raise ValueError(f"cloth_latents has spatial size {tuple(cloth_latents.shape[-2:])}, the server's latents "
                              f"{(self.h, self.w)}")
         dev, f16, Tp = self.device, torch.float16, self.T_page
+        copied = self._page_copied.pop(p, None)
+        if copied is not None:                  # the page's write-through reads it: the refill waits on the device
+            torch.cuda.current_stream(dev).wait_event(copied)
+        self._page_rows[p] = T
         with nvtx_range(f"b200vton.garment_page_fill[{p}]"):
             x_g = torch.zeros((1, self.h, self.w, CIN_PAD), dtype=f16, device=dev)
             self.L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), x_g, c_off=0)
@@ -896,14 +995,19 @@ class SlotDenoiser(_CapturedStep):
         return (s, self.S + s) if self.do_cfg else (s,)
 
     def admit(self, s, latents, mask, masked_image_latents, pose_latents, cloth_latents, prompt_embeds, add_text_embeds,
-              add_time_ids, image_embeds, text_embeds_cloth, page=None):
+              add_time_ids, image_embeds, text_embeds_cloth, page=None, host_page=None):
         """Writes one request into slot s, and only its rows. latents [1,4,h,w]; mask [1,1,h,w]; masked_image_latents,
         pose_latents, cloth_latents [1,4,h,w]; prompt_embeds [n,77,X], add_text_embeds [n,P], add_time_ids [n,6],
         image_embeds [n,16,X] with n = 2 ([uncond ; cond]) under CFG, else 1 (mask, masked_image_latents and
         pose_latents may have n rows too); text_embeds_cloth [1,77,X]. Pool mode: `page` is the filled page of the
-        request's garment (cloth_latents and text_embeds_cloth are then not read)."""
+        request's garment (cloth_latents and text_embeds_cloth are then not read); with a host tier, `host_page`
+        instead is the host page the slot streams from, from step 0 on (its first row is copied here)."""
         L, dev, f16 = self.L, self.device, torch.float16
-        if self.P is not None and (page is None or not 0 <= page < self.P):
+        if host_page is not None:
+            if self.host is None or page is not None or not 0 <= host_page < self.Q:
+                raise ValueError(f"admit streams from a host page in [0, {self.Q}) of a host tier, instead of a device "
+                                 f"page: got host_page={host_page}, page={page}")
+        elif self.P is not None and (page is None or not 0 <= page < self.P):
             raise ValueError(f"pool mode: admit needs the page of the request's garment in [0, {self.P}), got {page}")
         for name, t in (("latents", latents), ("mask", mask), ("masked_image_latents", masked_image_latents),
                         ("pose_latents", pose_latents), ("cloth_latents", cloth_latents)):
@@ -933,6 +1037,9 @@ class SlotDenoiser(_CapturedStep):
             L.nchw_to_nhwc(cloth_latents[:1].to(dev, f16).contiguous(), self.x_g[s:s + 1], c_off=0)
             self.garment.encode_context(text_embeds_cloth[:1].to(dev, f16),
                                         out=[(kv[s:s + 1], None) for kv, _ in self.ctx_g])
+        elif host_page is not None:
+            self.page[s], self.host_page[s] = None, int(host_page)
+            self._stream_rows([(s, 0)], after_last_step=True)
         else:
             self.page[s] = int(page)
         if self.x0_prev is not None:
@@ -947,18 +1054,111 @@ class SlotDenoiser(_CapturedStep):
         for r in self._rows(s):
             self.x_t[r].zero_()
         self.page[s] = None
+        self.host_page[s] = None
+
+    # ---- host tier --------------------------------------------------------------------------------
+    def _copy_streams(self):
+        """The host tier's side streams and the events that order them against the step: "ring" copies rows into the
+        ring (host to device), "write" copies filled pages to the host (device to host), so that a page's write-through
+        never holds up the next step's rows; "replayed": the last two replays' events (by replay parity); "ring_ready":
+        the ring copies the next replay waits for."""
+        if self._side is None:
+            ev = torch.cuda.Event
+            self._side = dict(ring=torch.cuda.Stream(device=self.device), write=torch.cuda.Stream(device=self.device),
+                              replayed=[ev(), ev()], n=0, ring_ready=ev(), ring_pending=False)
+        return self._side
+
+    def _stream_rows(self, loads, after_last_step):
+        """Copies host row q*T_page + i of each (slot, step i) in `loads` into ring row R + 2s + (i & 1) on the ring
+        stream, and makes the next replay wait for them. The ring stream first waits for the step that last read those
+        ring rows: the latest replay when a slot is admitted (after_last_step), else the one before it (the copies of
+        step i + 1 then run beside step i), and for a write-through into the host page still in flight."""
+        side = self._copy_streams()
+        stream = side["ring"]
+        k = side["n"] - (1 if after_last_step else 2)         # the replay to wait for (side["n"] replays so far)
+        if k >= 0:
+            stream.wait_event(side["replayed"][k & 1])
+        with torch.cuda.stream(stream):
+            for s, i in loads:
+                q = self.host_page[s]
+                written = self._host_written.get(q)
+                if written is not None:
+                    stream.wait_event(written)
+                src, dst = q * self.T_page + i, self.ring + 2 * s + (i & 1)
+                for pool_kv, host_kv in zip(self.pool, self.host.blocks):
+                    self._streamed[1] += copy_kv_rows(pool_kv, dst, host_kv, src)
+                self._streamed[0] += 1
+            side["ring_ready"].record(stream)
+        side["ring_pending"] = True
+
+    def write_through(self, p, q):
+        """Copies device page p (the rows of its last fill) to host page q on the write stream, after the work the
+        current stream has enqueued (the fill) and after the ring copies issued so far (which may read host page q's
+        previous garment). Until that copy is done, a refill of page p waits for it on the device, and rows streamed
+        from host page q wait for it on the ring stream. The host does not wait."""
+        if self.host is None or not (0 <= p < self.P and 0 <= q < self.Q) or p not in self._page_rows:
+            raise ValueError(f"write_through needs a host tier, a filled device page in [0, {self.P}) and a host page "
+                             f"in [0, {self.Q}): got {p}, {q}")
+        side = self._copy_streams()
+        stream = side["write"]
+        filled = torch.cuda.Event()
+        filled.record(torch.cuda.current_stream(self.device))
+        stream.wait_event(filled)
+        stream.wait_stream(side["ring"])
+        T, Tp = self._page_rows[p], self.T_page
+        with torch.cuda.stream(stream):
+            for host_kv, pool_kv in zip(self.host.blocks, self.pool):
+                copy_kv_rows(host_kv, q * Tp, pool_kv, p * Tp, T)
+            done = torch.cuda.Event()
+            done.record(stream)
+        self._page_copied[p] = self._host_written[q] = done
+
+    def take_streamed(self):
+        """(rows, bytes) copied from the host tier into the ring since the last call."""
+        out, self._streamed = tuple(self._streamed), [0, 0]
+        return out
+
+    def release_host(self):
+        """Waits for the side streams' copies, then unregisters and drops the host tier's memory."""
+        if self._side is not None:
+            self._side["ring"].synchronize()
+            self._side["write"].synchronize()
+        self._page_copied.clear()
+        self._host_written.clear()
+        if self.host is not None:
+            self.host.release()
+            self.host = None
 
     def _gkv_pre(self):
         return None if self.P is None else (self.pool, self.rows)
 
     def step(self, steps, noises=None, use_graph=True):
         """One denoise step of every occupied slot. steps: per slot, its request's step index or None (idle); noises:
-        {slot: [1,4,h,w] variance noise} for the slots whose scheduler step applies one. Returns the latents [S,4,h,w]."""
+        {slot: [1,4,h,w] variance noise} for the slots whose scheduler step applies one. Returns the latents [S,4,h,w].
+        With a host tier, the next row of every streaming slot is then copied into its ring beside the next step."""
         if self.ctx_t is None:
             raise RuntimeError("SlotDenoiser.step before any admission")
-        return self._run(use_graph, "b200vton.slot_denoise_step", steps, noises)
+        out = self._run(use_graph, "b200vton.slot_denoise_step", steps, noises)
+        if self.host is not None and self._side is not None:
+            side = self._side
+            side["replayed"][side["n"] & 1].record(torch.cuda.current_stream(self.device))
+            side["n"] += 1
+            loads = []
+            for s, e in enumerate(steps):
+                if e is None or self.host_page[s] is None:
+                    continue
+                i = int(e) if self.plans is None else int(e[1])
+                T = self.T if self.plans is None else self.plans[e[0]].T
+                if i + 1 < T:
+                    loads.append((s, i + 1))
+            if loads:
+                self._stream_rows(loads, after_last_step=False)
+        return out
 
     def _upload(self, steps, noises):
+        if self._side is not None and self._side["ring_pending"]:     # the ring rows this step reads
+            torch.cuda.current_stream(self.device).wait_event(self._side["ring_ready"])
+            self._side["ring_pending"] = False
         self.gather(steps)
         self.noise.zero_()
         for s, n in (noises or {}).items():

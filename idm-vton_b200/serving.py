@@ -536,6 +536,11 @@ class TryOnServer:
         return out
 
 
+# ContinuousTryOnServer.stats of the garment K/V pool's host tier
+HOST_STATS = ("garment_host_hits", "garment_host_writes", "garment_host_skipped", "garment_host_evictions",
+              "garment_rows_streamed", "garment_bytes_streamed")
+
+
 def _freeu(pipe):
     """The FreeU values the pipeline's try-on UNet runs with (enable_freeu, all four non-zero), or None."""
     return active_freeu(getattr(pipe.unet, "freeu", None))
@@ -570,6 +575,16 @@ class ContinuousTryOnServer:
         share its page; a retired request unpins it and the page stays resident, so a later request for that garment
         runs no garment pass at all. The step is then the try-on UNet only. P < slots is refused (ValueError naming the
         page size) before any launch. `stats` counts garment_page_fills and garment_page_hits.
+      * garment_kv_host_bytes=M beside garment_kv_bytes (pool mode with a host tier): Q = M // page_bytes more pages in
+        page-locked host memory, in the pool's format (denoise.HostGarmentKV), with an LRU of their own. Admission looks
+        a garment up on the device (pin the page), then on the host (the slot streams host page q, pinned there: each
+        step's row is copied into a ring of two device rows per slot beside the step before, SlotDenoiser), then fills
+        a device page and writes it through to a host page on a side stream (skipped and counted when every host page
+        is pinned). A device page whose write-through is in flight is refilled only after it, on the device. A host
+        hit is not copied back to a device page. Refused before any launch: garment_kv_host_bytes without
+        garment_kv_bytes and a host budget below one page (ValueError), and a failed page-lock (RuntimeError naming the
+        bytes). close() unregisters the host memory. `stats` adds garment_host_hits, garment_host_writes,
+        garment_host_skipped, garment_host_evictions, garment_rows_streamed and garment_bytes_streamed.
 
     RNG: each request owns a generator seeded with `req.seed` (the server's seed when None; unseeded when both are None)
     and draws in the order the pipeline draws for a batch of one: the initial noise, the masked image's VAE sample, the
@@ -592,9 +607,11 @@ class ContinuousTryOnServer:
 
     def __init__(self, pipe, height=1024, width=768, slots=4, num_inference_steps=30, guidance_scale=2.0, seed=None,
                  output_type="pt", eta=0.0, garment_kv_bytes=None, presets=None, default_preset=None,
-                 photo_filter="bicubic"):
+                 photo_filter="bicubic", garment_kv_host_bytes=None):
         from .photo import _check_filter
         _check_filter(photo_filter)
+        if garment_kv_host_bytes is not None and garment_kv_bytes is None:
+            raise ValueError("garment_kv_host_bytes is a host tier of the garment K/V pool: it needs garment_kv_bytes")
         self.photo_filter = photo_filter
         self.pipe = pipe
         self.height, self.width = height, width
@@ -620,6 +637,10 @@ class ContinuousTryOnServer:
         self.page_of = collections.OrderedDict()     # pool mode: garment_id -> page, least recently admitted first
         self.pins = collections.Counter()            # pool mode: page -> slots whose request reads it
         self.free_pages = []
+        self.garment_kv_host_bytes = None if garment_kv_host_bytes is None else int(garment_kv_host_bytes)
+        self.host_page_of = collections.OrderedDict()    # host tier: key -> host page, least recently used first
+        self.host_pins = collections.Counter()           # host tier: host page -> slots streaming from it
+        self.free_host_pages = []
         self.last_latents = {}                       # ticket -> final latents of the requests the last step() finished
         self._next_ticket = 0
         self.stats = collections.Counter()
@@ -648,9 +669,34 @@ class ContinuousTryOnServer:
         return len(self.waiting) + sum(e is not None for e in self.slots)
 
     # ---------------------------------------------------------------------------------------------
-    def _make_denoiser(self, pages=None):
+    def _make_denoiser(self, pages=None, **host):
         from .denoise import SlotDenoiser
-        return SlotDenoiser(self.pipe.unet.engine(), self.pipe.unet_encoder.engine(), self.S, pages=pages)
+        return SlotDenoiser(self.pipe.unet.engine(), self.pipe.unet_encoder.engine(), self.S, pages=pages, **host)
+
+    def _new_pool(self, T):
+        """Pool mode: a denoiser with a pool of pages of T rows and, with garment_kv_host_bytes, a host tier; every
+        refusal comes first."""
+        P, Q = self._pages(T), self._host_pages(T)
+        self.den = self._make_denoiser(pages=P) if Q is None else self._make_denoiser(pages=P, host_pages=Q)
+        self._reset_pages(P, Q)
+        if Q is not None:                            # the host tier's counters, shown from the first admission
+            self.stats.update(dict.fromkeys(HOST_STATS, 0))
+
+    def _drop_denoiser(self):
+        """Drops the denoiser; its host tier's memory is unregistered first."""
+        release = getattr(self.den, "release_host", None)
+        if release is not None:
+            release()
+        self.den = None
+
+    def close(self):
+        """Releases the garment K/V pool and unregisters the host tier's page-locked memory. The server stays usable:
+        the next admission configures it again (with empty pages). Refused while requests run."""
+        if any(e is not None for e in self.slots):
+            raise RuntimeError("close() while requests run in slots")
+        self._drop_denoiser()
+        self._configured = False
+        self._reset_pages(0)
 
     def page_bytes(self, T=None):
         """Pool mode: bytes of one garment's page, the hoisted K/V of all T steps at Bg = 1 (from the shapes). T defaults
@@ -671,10 +717,25 @@ class ContinuousTryOnServer:
                              f"least one page per slot ({self.S}, i.e. {self.S * page} bytes)")
         return P
 
-    def _reset_pages(self, P):
+    def _host_pages(self, T):
+        """Host tier: the number of pages its budget holds (None without a host tier); refuses less than one."""
+        if self.garment_kv_host_bytes is None:
+            return None
+        page = self.page_bytes(T)
+        Q = self.garment_kv_host_bytes // page
+        if Q < 1:
+            raise ValueError(f"garment_kv_host_bytes={self.garment_kv_host_bytes} holds no garment K/V page of {page} "
+                             f"bytes ({page / 1e9:.2f} GB: {T} steps at latent size {self.latent_size}); the host tier "
+                             "needs at least one page")
+        return Q
+
+    def _reset_pages(self, P, Q=None):
         self.page_of.clear()
         self.pins.clear()
         self.free_pages = list(range(P))
+        self.host_page_of.clear()
+        self.host_pins.clear()
+        self.free_host_pages = list(range(Q or 0))
 
     def _preset(self, name):
         p = self.presets[name]
@@ -712,9 +773,7 @@ class ContinuousTryOnServer:
             if self.garment_kv_bytes is None:
                 self.den = self._make_denoiser()
             else:
-                P = self._pages(len(timesteps))
-                self.den = self._make_denoiser(pages=P)
-                self._reset_pages(P)
+                self._new_pool(len(timesteps))
         self.den.configure(self._schedulers[name] or pipe.scheduler, timesteps, *self.latent_size,
                            guidance_scale=p.guidance_scale, do_cfg=pipe.do_classifier_free_guidance, eta=p.eta,
                            guidance_rescale=self.guidance_rescale)
@@ -743,9 +802,7 @@ class ContinuousTryOnServer:
             if self.garment_kv_bytes is None:
                 self.den = self._make_denoiser()
             else:
-                P = self._pages(T_max)
-                self.den = self._make_denoiser(pages=P)
-                self._reset_pages(P)
+                self._new_pool(T_max)
         self.den.configure_presets(self.plans, *self.latent_size, do_cfg=do_cfg)
         self.T = T_max
         self._configured = True
@@ -872,7 +929,8 @@ class ContinuousTryOnServer:
             if any(e is not None for e in self.slots):
                 raise RuntimeError(f"the pipeline's garment K/V precision changed to {fmt!r} while requests run in "
                                    f"{self._kv_format!r}: change it when the server is idle")
-            self.den, self._configured = None, False
+            self._drop_denoiser()
+            self._configured = False
         if not getattr(self, "_configured", False):
             self._configure()
             self._kv_format = fmt
@@ -902,17 +960,41 @@ class ContinuousTryOnServer:
                     key = (req.garment_id, tuple(float(t) for t in t_table))
                 else:
                     j, T, t_table, key = None, self.T, None, req.garment_id
-                page = None if self.garment_kv_bytes is None else self._pin_page(key, g, t_table)
+                page, host = (None, None) if self.garment_kv_bytes is None else self._pin_garment(key, g, t_table)
                 self.den.admit(s, cloth_latents=g["latents"], image_embeds=g["image_embeds"],
-                               text_embeds_cloth=g["text_embeds_cloth"], page=page, **prep)
+                               text_embeds_cloth=g["text_embeds_cloth"], page=page,
+                               **({} if host is None else dict(host_page=host)), **prep)
                 self.slots[s] = dict(req=req, gen=gen, step=0, page=page, plan=j, T=T, photo=entry)
+                if host is not None:
+                    self.slots[s]["host_page"] = host
                 self.stats["admitted"] += 1
             free = [s for s, e in enumerate(self.slots) if e is None]
+        self._count_streamed()
+
+    def _count_streamed(self):
+        if self.garment_kv_host_bytes is not None and self.den is not None:
+            rows, nbytes = self.den.take_streamed()
+            self.stats["garment_rows_streamed"] += rows
+            self.stats["garment_bytes_streamed"] += nbytes
+
+    def _pin_garment(self, key, g, t_table=None):
+        """Pool mode: (device page, None) or, with a host tier, (None, host page) holding `key`, pinned for one more
+        slot. Lookup order: a device page; a host page (the slot streams from it and pins no device page, so P >= slots
+        still holds for the device pages); then a miss (_pin_page)."""
+        if self.garment_kv_host_bytes is not None and key not in self.page_of:
+            q = self.host_page_of.get(key)
+            if q is not None:
+                self.host_page_of.move_to_end(key)
+                self.host_pins[q] += 1
+                self.stats["garment_host_hits"] += 1
+                return None, q
+        return self._pin_page(key, g, t_table), None
 
     def _pin_page(self, key, g, t_table=None):
         """Pool mode: the page holding `key` (the garment id; with the mixed-kind step, (garment id, the plan's
         timesteps t_table)), pinned for one more slot. A miss fills a free page, else the least recently admitted
-        unpinned one (one exists: a free slot means at most slots - 1 pinned pages, and P >= slots)."""
+        unpinned one (one exists: a free slot means at most slots - 1 pinned pages, and P >= slots), and with a host
+        tier writes it through to a host page."""
         p = self.page_of.get(key)
         if p is not None:
             self.page_of.move_to_end(key)
@@ -927,8 +1009,26 @@ class ContinuousTryOnServer:
             self.den.fill_page(p, g["latents"], g["text_embeds_cloth"], *(() if t_table is None else (t_table,)))
             self.page_of[key] = p
             self.stats["garment_page_fills"] += 1
+            if self.garment_kv_host_bytes is not None:
+                self._write_through(key, p)
         self.pins[p] += 1
         return p
+
+    def _write_through(self, key, p):
+        """Host tier: device page p, just filled with `key`, copied to a free host page, else to the least recently used
+        unpinned one; skipped (and counted) when every host page is pinned. The device page is valid either way."""
+        if self.free_host_pages:
+            q = self.free_host_pages.pop(0)
+        else:
+            victim = next((k for k, q in self.host_page_of.items() if self.host_pins[q] == 0), None)
+            if victim is None:
+                self.stats["garment_host_skipped"] += 1
+                return
+            q = self.host_page_of.pop(victim)
+            self.stats["garment_host_evictions"] += 1
+        self.den.write_through(p, q)
+        self.host_page_of[key] = q
+        self.stats["garment_host_writes"] += 1
 
     def _decode(self, latents):
         if self.output_type == "latent":
@@ -966,6 +1066,7 @@ class ContinuousTryOnServer:
                 noises[s] = n
         steps = [None if e is None else e["step"] if e["plan"] is None else (e["plan"], e["step"]) for e in self.slots]
         latents = den.step(steps, noises, use_graph=use_graph and getattr(self.pipe, "use_cuda_graph", True))
+        self._count_streamed()
         self.stats["steps"] += 1
         self.stats["slot_steps"] += len(active)
         done = []
@@ -990,6 +1091,8 @@ class ContinuousTryOnServer:
             den.release(s)
             if self.slots[s]["page"] is not None:      # the page stays resident as a cache entry
                 self.pins[self.slots[s]["page"]] -= 1
+            if self.slots[s].get("host_page") is not None:
+                self.host_pins[self.slots[s]["host_page"]] -= 1
             self.slots[s] = None
         self.stats["images"] += len(done)
         return {t: images[i] for i, t in enumerate(tickets)}
